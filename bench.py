@@ -1,13 +1,16 @@
 #!/usr/bin/env python
 """Benchmark of the stylization hot path (BASELINE.json metric: stylized frames/s @512x512).
 
-    python bench.py --gpus N --steps K --warmup W                 # this repo's B200 engine, BASELINE configs[1]
+    python bench.py --gpus N --steps K --warmup W                 # this repo's engine, BASELINE configs[1]
+    python bench.py ... --dump-outputs DIR                        # also write the last timed step's outputs as .npy
     python bench.py --config c3|c4|c5 --gpus N ...                # the other BASELINE configs (528^2 / 8 characters / 1024^2 stage 1)
     python bench.py --impl reference --gpus N --steps K ...       # the reference's CPU path (oracle port) on the host cores
 
 One *step* = one pass of stage 1 -> uint8 -> edge burn-in -> stage 2 -> uint8 RGBA over the rank's synthetic
 frame stack.  With N > 1 (torchrun, one rank per GPU) every rank owns its own frame range, weights are broadcast
-once over NCCL and there is no per-frame collective.  Prints ONE JSON line on rank 0.
+once over NCCL and there is no per-frame collective.  Prints ONE JSON line on rank 0.  The synthetic inputs are
+seeded, so the same arguments give the same inputs on every run; ``--dump-outputs DIR`` writes what the timed path
+returned in its last step (rank 0, float32, a fixed sample of frames) so that two builds can be compared output for output.
 
 What the line reports (round-2 contract):
 * ``value`` / ``e2e`` / ``roofline``: the PARITY-GRADE mode (split-fp16 "fp16x3", <= 1e-3 max-abs against the fp32
@@ -16,7 +19,7 @@ What the line reports (round-2 contract):
   forward (the oracle port run on cuda with TF32 off), before anything is timed; a failing gate exits non-zero;
 * ``config.fast_mode``: the single-pass fp16 mode (same operand class as the reference's own default GPU path,
   which runs its convolutions in TF32 = 10-bit mantissa) with its measured error, fps, e2e and roofline;
-* ``config.gpu_baseline``: the reference's forward on the same B200 (torch cuDNN + torchvision deform_conv2d CUDA
+* ``config.gpu_baseline``: the reference's forward on the same GPU (torch cuDNN + torchvision deform_conv2d CUDA
   kernels; batch 1 as test_stage1.py:57-63 runs it, and batch 16), fps and its own error against true fp32;
 * ``cpu_baseline``: the reference's CPU path on the host cores, bounded sample.
 """
@@ -37,6 +40,7 @@ if ROOT not in sys.path:
 METRIC = "stylized frames/sec @512x512 (stage1+stage2)"
 UNIT = "frames/s"
 TOL = 1e-3          # BASELINE.json north_star: max-abs fp32 against the reference's own forward
+DUMP_FRAMES = 8     # --dump-outputs: 8 RGBA frames of 512 x 512 as float32 = 32 MB, shared by the characters of the rank
 
 CONFIGS = {
     # name: (workload description, frame size, total frames (None = per-GPU), characters, stage-1 only, scaling)
@@ -55,7 +59,8 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return json.load(f), "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense FP16/BF16 989 TFLOP/s - a ceiling, not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "NVIDIA H100 SXM data sheet"
 
 
 def usable_cores():
@@ -324,6 +329,19 @@ def parity_gate(pipes, dev, size, sd1, sd2, seed):
     return res
 
 
+def dump_outputs(out_dir, outputs, size):
+    """--dump-outputs: per character, the RGBA uint8 frames the timed path returned, as float32 [n, H, W, 4] for a sample
+    of frames drawn with a fixed seed (rgba_char<c>.npy) and the indices of those frames (rgba_char<c>_frames.npy)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    n_keep = max(1, DUMP_FRAMES * 512 * 512 // (size * size) // max(1, len(outputs)))     # <= 32 MB in all
+    for c, rgba in sorted(outputs.items()):
+        rng = np.random.default_rng(1000 + c)
+        idx = np.sort(rng.choice(rgba.shape[0], size=min(n_keep, rgba.shape[0]), replace=False))
+        np.save(os.path.join(out_dir, "rgba_char%d.npy" % c), rgba[idx.tolist()].cpu().numpy().astype(np.float32))
+        np.save(os.path.join(out_dir, "rgba_char%d_frames.npy" % c), idx.astype(np.float64))
+
+
 # ------------------------------------------------------------------------------------------------ engine arm
 def main():
     ap = argparse.ArgumentParser()
@@ -341,6 +359,9 @@ def main():
     ap.add_argument("--no-gpu-baseline", action="store_true")
     ap.add_argument("--no-fast", action="store_true", help="skip the secondary single-pass fp16 measurement")
     ap.add_argument("--no-parity-gate", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the RGBA frames the timed path returned in its last step (float32 .npy, a seeded sample "
+                         "of at most %d frames per character) to DIR" % DUMP_FRAMES)
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -365,7 +386,7 @@ def main():
     from drawingspinup_b200.pipeline import StylizationPipeline, assign_work, broadcast_state_dict
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device - the B200 engine has no CPU fallback (use --impl reference for the CPU path)")
+        raise SystemExit("bench.py: no CUDA device - the engine has no CPU fallback (use --impl reference for the CPU path)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -414,14 +435,17 @@ def main():
         return {c: StylizationPipeline(weights[c][0], None if stage1_only else weights[c][1], dev, precision=precision,
                                        batch=args.batch) for c in my_chars}
 
-    def measure(pipes, host: bool):
+    def measure(pipes, host: bool, last=None):
+        """Milliseconds of args.steps timed steps; `last` (a dict) receives each character's output of the last step."""
         def fn():
             for c in my_chars:
                 st = stacks[c]
                 if host:
-                    pipes[c].run_host(*st["host"], st["out"])
+                    r = pipes[c].run_host(*st["host"], st["out"])
                 else:
-                    pipes[c].run(*st["dev"])
+                    r = pipes[c].run(*st["dev"])
+                if last is not None:
+                    last[c] = r
         for _ in range(args.warmup):
             fn()
         barrier()
@@ -437,8 +461,7 @@ def main():
         return ms.item()
 
     peaks, peak_kind = load_peaks()
-    peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1400.0)))
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0)))
 
     def layer_roofline(pipe, tensor_factor):
         """Per-launch device times of one batch (CUDA events around every launch on the launching stream) -> the
@@ -450,16 +473,9 @@ def main():
                 table.append({"kernel": tag + "." + name, "ms": ms, "tflops": (fl / (ms * 1e-3) / 1e12) if ms > 0 else 0.0,
                               "gflop": fl / 1e9})
         top = max(table, key=lambda r: r["ms"])
-        traffic, traffic_src = None, None
-        tpath = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tpath) and args.batch == 16 and S == 512:
-            with open(tpath) as f:
-                ent = json.load(f).get(top["kernel"] + (":x3" if tensor_factor == 3 else ""))
-            if ent:
-                traffic, traffic_src = ent["bytes"], ent["source"]
         roof = {"bound": "tensor", "kernel": top["kernel"], "achieved": top["tflops"], "peak": peak, "unit": "TFLOP/s",
-                "frac": top["tflops"] / peak, "traffic": traffic, "traffic_source": traffic_src,
-                "peak_source": "%s bf16_tflops_sustained (kernel timed inside a long step)" % peak_kind,
+                "frac": top["tflops"] / peak,
+                "peak_source": "%s (dense FP16/BF16 tensor rate)" % peak_kind,
                 "launch_ms": top["ms"], "launch_gflop": top["gflop"],
                 "achieved_definition": "algorithmic conv FLOPs of the launch (SURVEY 8d) / CUDA-event launch time",
                 "tensor_work_factor": tensor_factor,
@@ -495,8 +511,12 @@ def main():
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    ms_total = measure(pipes, host=False)
+    last_out = {}
+    ms_total = measure(pipes, host=False, last=last_out)
     clocks = sampler.stop() if rank == 0 else None
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, last_out, S)
+    del last_out
     ms_e2e = measure(pipes, host=True)
     fps = all_frames * args.steps / (ms_total / 1e3)
     fps_e2e = all_frames * args.steps / (ms_e2e / 1e3)
@@ -563,9 +583,9 @@ def main():
                            "batch_per_launch": args.batch, "characters": n_chars, "stages": "stage1" if stage1_only else "stage1+stage2",
                            "parallelism": ("character -> GPU x%d, no weight broadcast" % world) if n_chars > 1 else
                                           ("frame-shard x%d, weights broadcast once" % world),
-                           "l2": "inputs+activations per step (>2 GB) exceed the 126 MB L2; no explicit flush",
+                           "l2": "inputs+activations per step (>2 GB) exceed the 50 MB L2; no explicit flush",
                            "workspace_bytes_per_handle": workspace,
-                           "hbm_fraction_of_180GB": workspace * len(my_chars) / 180e9,
+                           "hbm_fraction_of_80GB": workspace * len(my_chars) / 80e9,
                            "gflop_per_frame": flops_frame / 1e9,
                            "parity": parity, "fast_mode": fast, "gpu_baseline": gpu_base},
                 "e2e": {"value": fps_e2e, "unit": UNIT, "h2d_bytes_per_step": int(all_frames * S * S * 9),

@@ -1,10 +1,10 @@
-"""drawingspinup_b200 - B200-native engine for DrawingSpinUp's per-frame stylization hot path.
+"""drawingspinup_b200 - CUDA (H100, sm_90a) engine for DrawingSpinUp's per-frame stylization hot path.
 
 Public surface (mirrors ``3_style_translator/training/models.py`` for the inference path):
 
 * :class:`GeneratorJ_RIC`, :class:`GeneratorJ` - drop-in classes for ``training.models``.
 * :func:`install` - rebind those two names inside the reference's ``training.models`` so that
-  ``training.trainers.build_model`` (trainers.py:33-35) builds the B200 engine.
+  ``training.trainers.build_model`` (trainers.py:33-35) builds the CUDA engine.
 * :mod:`drawingspinup_b200.pipeline` - device-resident stage-1 -> stage-2 frame pipeline with
   frame sharding across GPUs; :mod:`drawingspinup_b200.run` - launcher for the unmodified
   ``test_stage1.py`` / ``test_stage2.py``.
@@ -19,7 +19,7 @@ def install(models_module=None):
 
     ``build_model`` resolves the class by name at call time (``getattr(m, model_type)``,
     trainers.py:33-35), so after this call the unmodified reference scripts construct, load and
-    call the B200 engine.  Returns the patched module."""
+    call the CUDA engine.  Returns the patched module."""
     if models_module is None:
         import importlib
         models_module = importlib.import_module("training.models")

@@ -1,7 +1,7 @@
 """ctypes binding of ``libdsu_b200.so`` (C ABI in ``include/dsu_b200.h``).
 
-The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is no
-fallback: if the shared object is missing or the device is not a B200, calls raise.
+The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is no
+fallback: if the shared object is missing or the device is not an sm_90 GPU (H100), calls raise.
 """
 from __future__ import annotations
 
@@ -41,7 +41,6 @@ SYMBOLS = {
     "dsu_loaded_keys": (C.c_int, [_VP]),
     "dsu_finalize": (C.c_int, [_VP, _VP]),
     "dsu_set_knob": (C.c_int, [_VP, C.c_char_p, _I32]),
-    "dsu_debug_watchdog": (C.c_int, [_VP, C.POINTER(C.c_uint64), _I32]),
     "dsu_set_ric_offsets": (C.c_int, [_VP, _I32, _I32, _VP]),
     "dsu_forward": (C.c_int, [_VP, _VP, _I32, _I32, _I32, _VP, _VP]),
     "dsu_forward_u8": (C.c_int, [_VP, _VP, _VP, _VP, _I32, _I32, _I32, _VP, _VP, _VP]),
@@ -69,7 +68,7 @@ def lib() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 "drawingspinup_b200: %s is missing - build it with `python -c 'import __graft_entry__ as g; "
-                "g.build()'` (nvcc, sm_100a).  There is no CPU or PyTorch fallback." % LIB_PATH)
+                "g.build()'` (nvcc, sm_90a).  There is no CPU or PyTorch fallback." % LIB_PATH)
         handle = C.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
             fn = getattr(handle, name)

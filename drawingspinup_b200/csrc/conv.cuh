@@ -9,20 +9,12 @@ namespace dsu {
 
 constexpr int kTileH = 8;       // output patch rows per CTA
 constexpr int kTileW = 16;      // output patch cols per CTA
-constexpr int kTileM = 128;     // = UMMA M
+constexpr int kTileM = 128;     // output pixels per CTA = two warpgroups x wgmma M = 64
 constexpr int kChunkK = 64;     // fp16 K elements per smem row (128 B, SWIZZLE_128B)
 constexpr int kABytes = kTileM * 128;   // bytes of one A stage
-constexpr int kWorkers = 256;   // producer / epilogue threads (warps 0-7)
-// A single warp sustains only ~100 cycles per tcgen05.mma in SS mode (tools/umma_rate.cu), far above the
-// 32/64-cycle execution time of an M=128, N=64/128, K=16 MMA, so a CTA runs several issuing warps, each
-// with its own TMEM accumulator (sub-tile and/or K split; partial sums are added in the epilogue).
-constexpr int kIssuersTap = 1;   // tap-mode plain conv
-constexpr int kIssuersHalo = 4;  // halo: ns sub-tiles x ks K-splits <= 4 (8 issuers with 4 worker warps measured slower)
-constexpr int kThreadsTap = (8 + kIssuersTap + 1) * 32;
-constexpr int kThreadsHalo = (8 + kIssuersHalo + 1) * 32;
+constexpr int kThreads = 256;   // two warpgroups: producers, MMA issuers and epilogue alike
+constexpr int kStages = 4;      // A + B ring depth; chunk q + 2 is loaded while the MMAs of chunk q run
 constexpr int kMaxSeg = 6;      // concat segments (second half = lo planes in exact mode)
-constexpr int kMaxStagesA = 9;  // RIC keeps one A buffer per tap resident
-constexpr int kMaxStagesB = 16;
 
 // One 16-byte (8-channel) K slot: which tap of which source segment fills it.
 // plain conv: one entry per (chunk, slot).  RIC conv: one entry per (64-channel block, slot) - the
@@ -36,15 +28,12 @@ struct Slot {
 };
 static_assert(sizeof(Slot) == 8, "Slot must be 8 bytes");
 
-// Host-side description of one K chunk (8 slots = 64 K elements) of the implicit GEMM; the kernels get the masks as
-// launch constants (kmask_full / kmask_last) and the tile offset as chunk_index * b_bytes.
+// Host-side description of one K chunk (8 slots = 64 K elements) of the implicit GEMM; the kernel gets the masks as
+// launch constants (kmask_full / kmask_last).
 struct ChunkHdr {
-    uint8_t kmask;      // which of the 4 UMMA K=16 steps are issued against B tile 0
+    uint8_t kmask;      // which of the 4 K=16 steps are issued against B tile 0
     uint8_t kmask2;     // exact mode: which of A steps 0-1 (the hi half) are issued against B steps 2-3 (W_lo)
-    uint16_t pad_;
-    uint32_t b_off;     // byte offset of this chunk's B tile(s) inside wpack
 };
-static_assert(sizeof(ChunkHdr) == 8, "ChunkHdr must be 8 bytes");
 
 struct Seg {
     const __half* ptr;
@@ -85,21 +74,12 @@ struct ConvParams {
     int Hin, Win;           // source buffer geometry (before the fused nearest x2)
     int Hv, Wv;             // virtual conv-input geometry = (Hin << up, Win << up)
     int stride, up, ric, exact;
-    int nchunks, nblocks, Cout, sa, sb, tmem_cols;
-    int b_bytes;            // bytes per B stage = bytes of one chunk's weight tile(s) in wpack
-    // K-step masks (ChunkHdr semantics) as launch constants so the issuing warp stays uniform:
-    // every chunk uses *_full except the ragged tail (tap mode: the last chunk; block modes: all
-    // chunks of the last channel block), which uses *_last
+    int nchunks, nblocks, Cout;
+    int b_bytes;            // bytes per B stage = Cout x 128 (one chunk's weight tile in wpack)
+    // K-step masks (ChunkHdr semantics) as launch constants so the issuing warpgroups stay uniform:
+    // every chunk uses *_full except the ragged tail (tap mode: the last chunk; RIC: all chunks of the last
+    // channel block), which uses *_last
     uint32_t kmask_full, kmask_last, kmask2_full, kmask2_last;
-    // halo mode (plain stride-1 convs): one (16+2p) x (8*ns+2p) pixel halo tile per 64-channel block
-    // is staged once and every tap reads a shifted window of it through the UMMA descriptor
-    int halo, ns, ks, ksize, pad, halo_w, halo_rows, halo_bytes;   // ks: K-split issuers per sub-tile
-    int tps;                // persistent halo kernel: taps per weight stage (one bulk copy / one commit per tps taps)
-    // split-fp16 halo layers with Cout = 64: the weight tile of a (tap, 32-channel block) is a no-swizzle K-major tile of 128
-    // rows [W_hi (64) ; W_lo (64)] x 32 channels, so a_hi x [W_hi | W_lo] is ONE N = 128 MMA (64 cycles, inside the shared-
-    // memory operand bandwidth) and a_lo x W_hi one N = 64 MMA on the first 64 rows: 113 instead of 3 x 49 cycles per K16
-    // step.  Accumulator = 128 columns per issuer (hi.W_hi + lo.W_hi | hi.W_lo), summed by the epilogue.  nsets: 1 or 2.
-    int n128, nsets;
     const Slot* slots;      // plain: [nchunks][8]; RIC: [nblocks][8]
     const uint8_t* wpack;   // pre-swizzled B tiles
     Seg seg[kMaxSeg];
@@ -109,50 +89,17 @@ struct ConvParams {
     const uint8_t* ric_oct; // [Hout*Wout]
     const uint2* ric_wh;    // [Hout*Wout][8] the 4 bilinear weights of each rotated tap as fp16 {w00,w01 | w10,w11} (packed-half2 blend)
     EpiParams epi;
-    // sub-pixel class of a fused nearest-x2 + 3x3 convolution (experimental, DSU_SUBPIXEL=1; conv_halo_persist_kernel<true>):
-    // the launch is a 2x2 convolution over the LOW-resolution source with asymmetric padding (pad_y, pad_x) whose output
-    // pixel (oy, ox) of the Hout x Wout grid lands at (2*oy + sub_py, 2*ox + sub_px) of the (2*Hout) x (2*Wout) output buffer
-    int sub, sub_py, sub_px, pad_y, pad_x;
+    // sub-pixel class of a fused nearest-x2 + 3x3 convolution: the launch is a 2x2 convolution over the LOW-resolution
+    // source whose output pixel (oy, ox) of the Hout x Wout grid lands at (2*oy + sub_py, 2*ox + sub_px) of the
+    // (2*Hout) x (2*Wout) output buffer
+    int sub, sub_py, sub_px;
+    // first layer (one 8-channel segment, stride 1): stage the (kTileH + ksize - 1) x (kTileW + ksize - 1) input halo of the
+    // tile once in shared memory and build every A chunk from it instead of from global memory
+    int halo, ksize, pad;
+    int n128;               // Cout a multiple of 128: issue N = 128 wgmma instructions (else N = 64 / 32)
 };
-
-// ---------------------------------------------------------------------------------------------------------------------------
-// RIC convolution with the A operand in TENSOR MEMORY (conv_ric_tm.cu): the stage-1 kernel of round 2.
-// A "block" is what one TMA tensor load stages: 128 bytes of source channels per halo pixel (64 fp16 channels, or 32 fp32
-// channels in split-fp16 mode) from one contiguous channel run of one buffer; it feeds up to two "stages" of 4 16-byte
-// chunks each.  A stage is one hand-off unit: 144 TMEM columns of blended taps + its weight tiles + one commit.
-constexpr int kTmMaxBlocks = 12;
-constexpr int kTmMaxMaps = 3;
-constexpr int kTmStageCols = 144;        // 9 taps x 2 parts x 8 columns (fp16: two K16 steps; split-fp16: hi and lo of one K16 step)
-constexpr int kTmHaloBytes = 23552;      // 18 x 10 pixel lines of 128 B, rounded up to the 1024-byte swizzle atom
-constexpr int kTmProducerWarps = 8, kTmEpilogueWarps = 4, kTmIssuerWarps = 6, kTmLoaderWarps = 2;
-constexpr int kTmThreads = (kTmProducerWarps + kTmEpilogueWarps + kTmIssuerWarps + kTmLoaderWarps) * 32;
-struct TmBlock {
-    uint8_t map;            // tensor map (channel run) index
-    uint8_t nstages;        // stages of this block that carry weights (1 or 2)
-    uint8_t chunks[2];      // 16-byte chunks with real channels per stage (1..4); the rest reads zeros
-    uint16_t c0;            // first channel of the block inside its run (elements)
-    uint16_t pad_;
-};
-struct TmParams {
-    ConvParams c;           // output geometry, stencil tables and the epilogue (shared with the other kernels)
-    alignas(64) CUtensorMap tmap[kTmMaxMaps];
-    TmBlock blk[kTmMaxBlocks];
-    int nblocks, nstages;   // per tile
-    int sa, sb, nsets, ni;  // TMEM A stages, weight stages in shared memory (multiple of sa), accumulator sets, issuing warps
-    int halo_w, halo_h;     // 18 x 10 (or 10 x 6 with the fused nearest x2)
-    int b_stage_bytes;      // Cout * 576: 9 taps x 2 parts x (Cout x 32 B no-swizzle tile)
-    const uint8_t* wpack;   // [stage][tap][part][Cout x 32 B]
-    unsigned long long* dbg;    // watchdog records (pinned host memory, one slot per warp) or null
-    unsigned long long* trace;  // development trace (knob tm_trace): 5 x 1024 (event, clock) records of CTA 0, or null
-};
-cudaError_t launch_conv_ric_tm(const TmParams& p, cudaStream_t stream);
-size_t conv_ric_tm_smem_bytes(int cout, int sb);
 
 cudaError_t launch_conv(const ConvParams& p, cudaStream_t stream);
-cudaError_t launch_conv_halo_persist(const ConvParams& p, cudaStream_t stream);
-// first-layer kernel (conv_first.cu): reuses sa = halo buffers, ks = issuers, ns = accumulator sets, ksize / pad / halo_rows / halo_bytes
-cudaError_t launch_conv_first(const ConvParams& p, cudaStream_t stream);
-size_t conv_halo_smem_bytes(const ConvParams& p);
 size_t conv_smem_bytes(const ConvParams& p);
 
 }  // namespace dsu

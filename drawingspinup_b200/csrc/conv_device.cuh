@@ -1,5 +1,5 @@
 // Device helpers shared by the convolution kernels: fp16 pack/split, the exact uint8 conversion and
-// the fused epilogue (TMEM accumulator row -> BN/activation/residual -> fp16 NHWC / fp32 / uint8).
+// the fused epilogue (accumulator row -> BN/activation/residual -> fp16 NHWC / fp32 / uint8).
 #pragma once
 #include "conv.cuh"
 #include "ptx.cuh"
@@ -56,60 +56,32 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
 }
 
 // 32 channels of one pixel -> fp16 NHWC (hi plane, plus the split-fp16 lo plane when kLo and `lo` is non-null)
-// kWide = false: 128-bit stores only.  (The tensor-memory RIC kernel runs its epilogue in a non-inlined, register-tight
-// function; there ptxas 12.9 assembled the predicated st.global.v8.b32 of one instantiation as a plain 32-bit STG - only the
-// first word of every 32 bytes reached memory, found as "channels 0,1 of each batch correct, the rest zero".)
-template <bool kLo, bool kWide = true>
+template <bool kLo>
 __device__ __forceinline__ void store32(__half* hi, __half* lo, const float* f) {
-    // 32-byte aligned destinations (every buffer whose pixel pitch and channel offset are multiples of 16 channels) take
-    // two 256-bit stores.  The choice is made warp-uniform (a 40-channel pitch aligns only every other pixel): the epilogue's
-    // tcgen05.ld / tcgen05.st are warp-collective and must never be reached by a diverged warp
-    const bool wide = kWide && __all_sync(__activemask(), (reinterpret_cast<uintptr_t>(hi) & 31u) == 0);   // (lanes of pixels outside the image are not here)
     if (kLo && lo) {
         uint4 h[4], l[4];
 #pragma unroll
         for (int c = 0; c < 4; ++c) split8(f + 8 * c, h[c], l[c]);
-        if (wide) {
-            st_global_256(hi, h[0], h[1]); st_global_256(hi + 16, h[2], h[3]);
-            st_global_256(lo, l[0], l[1]); st_global_256(lo + 16, l[2], l[3]);
-        } else {
 #pragma unroll
-            for (int c = 0; c < 4; ++c) { reinterpret_cast<uint4*>(hi)[c] = h[c]; reinterpret_cast<uint4*>(lo)[c] = l[c]; }
-        }
+        for (int c = 0; c < 4; ++c) { reinterpret_cast<uint4*>(hi)[c] = h[c]; reinterpret_cast<uint4*>(lo)[c] = l[c]; }
     } else {
-        uint4 h[4];
 #pragma unroll
-        for (int c = 0; c < 4; ++c) h[c] = pack8(f + 8 * c);
-        if (wide) {
-            st_global_256(hi, h[0], h[1]); st_global_256(hi + 16, h[2], h[3]);
-        } else {
-#pragma unroll
-            for (int c = 0; c < 4; ++c) reinterpret_cast<uint4*>(hi)[c] = h[c];
-        }
+        for (int c = 0; c < 4; ++c) reinterpret_cast<uint4*>(hi)[c] = pack8(f + 8 * c);
     }
 }
 
-// 32 channels of one pixel -> fp32 NHWC (stage-1 activations of the split-fp16 mode); 32-byte aligned rows take 256-bit stores
-template <bool kWide = true>
+// 32 channels of one pixel -> fp32 NHWC (stage-1 activations of the split-fp16 mode)
 __device__ __forceinline__ void store32_f32(float* dst, const float* f) {
-    if (kWide && __all_sync(__activemask(), (reinterpret_cast<uintptr_t>(dst) & 31u) == 0)) {      // warp-uniform, see store32
 #pragma unroll
-        for (int c = 0; c < 4; ++c)
-            st_global_256(dst + 8 * c, make_uint4(__float_as_uint(f[8 * c]), __float_as_uint(f[8 * c + 1]), __float_as_uint(f[8 * c + 2]), __float_as_uint(f[8 * c + 3])),
-                          make_uint4(__float_as_uint(f[8 * c + 4]), __float_as_uint(f[8 * c + 5]), __float_as_uint(f[8 * c + 6]), __float_as_uint(f[8 * c + 7])));
-    } else {
-#pragma unroll
-        for (int c = 0; c < 8; ++c) reinterpret_cast<float4*>(dst)[c] = make_float4(f[4 * c], f[4 * c + 1], f[4 * c + 2], f[4 * c + 3]);
-    }
+    for (int c = 0; c < 8; ++c) reinterpret_cast<float4*>(dst)[c] = make_float4(f[4 * c], f[4 * c + 1], f[4 * c + 2], f[4 * c + 3]);
 }
 
 // One 32-column batch of one accumulator row after the K-split partial sums were added: folded BN / bias, activation,
 // optional post-activation affine, residual stream, fp16 stores, conv_12 partial dot products.  The activation, the
-// second affine and the lo plane are compile-time (dispatched once per row in epilogue_row): with run-time tests inside
-// the 32-element loops a batch cost ~210 instructions (113 of them branches) on a latency-bound lone warp
-// (profiles/r01m_conv_first.ncu-rep), this form ~70 + the stores.
-template <int kAct, int kScale2, bool kLo, bool kWide = true>   // kAct / kScale2 = -1: decided at run time (cold generic variant)
-__device__ __forceinline__ void epilogue_batch(const ConvParams& p, const float* s_par, const uint32_t* v, size_t opix, int cb,
+// second affine and the lo plane are compile-time (dispatched once per row in epilogue_row), which keeps run-time tests
+// out of the 32-element loops.
+template <int kAct, int kScale2, bool kLo>   // kAct / kScale2 = -1: decided at run time (cold generic variant)
+__device__ __forceinline__ void epilogue_batch(const ConvParams& p, const float* s_par, const float* v, size_t opix, int cb,
                                                bool tail, float* y3) {
     const EpiParams& e = p.epi;
     const int C = p.Cout;
@@ -120,10 +92,10 @@ __device__ __forceinline__ void epilogue_batch(const ConvParams& p, const float*
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
             const float4 a = sc[q], b = sh[q];
-            f[4 * q] = fmaf(__uint_as_float(v[4 * q]), a.x, b.x);
-            f[4 * q + 1] = fmaf(__uint_as_float(v[4 * q + 1]), a.y, b.y);
-            f[4 * q + 2] = fmaf(__uint_as_float(v[4 * q + 2]), a.z, b.z);
-            f[4 * q + 3] = fmaf(__uint_as_float(v[4 * q + 3]), a.w, b.w);
+            f[4 * q] = fmaf(v[4 * q], a.x, b.x);
+            f[4 * q + 1] = fmaf(v[4 * q + 1], a.y, b.y);
+            f[4 * q + 2] = fmaf(v[4 * q + 2], a.z, b.z);
+            f[4 * q + 3] = fmaf(v[4 * q + 3], a.w, b.w);
         }
     }
     const int act = kAct >= 0 ? kAct : e.act;
@@ -159,17 +131,17 @@ __device__ __forceinline__ void epilogue_batch(const ConvParams& p, const float*
 #pragma unroll
         for (int c = 0; c < 8; ++c) rp[c] = make_float4(f[4 * c], f[4 * c + 1], f[4 * c + 2], f[4 * c + 3]);
     }
-    if (e.out2_f32) store32_f32<kWide>(e.out2_f32 + opix * e.out2_pitch + e.out2_choff + cb, f);
+    if (e.out2_f32) store32_f32(e.out2_f32 + opix * e.out2_pitch + e.out2_choff + cb, f);
     else if (e.out2_hi)
-        store32<kLo, kWide>(e.out2_hi + opix * e.out2_pitch + e.out2_choff + cb,
+        store32<kLo>(e.out2_hi + opix * e.out2_pitch + e.out2_choff + cb,
                      e.out2_lo ? e.out2_lo + opix * e.out2_pitch + e.out2_choff + cb : nullptr, f);
     if (e.out_relu) {
 #pragma unroll
         for (int c = 0; c < 32; ++c) f[c] = fmaxf(f[c], 0.0f);
     }
-    if (e.out_f32) store32_f32<kWide>(e.out_f32 + opix * e.out_pitch + e.out_choff + cb, f);
+    if (e.out_f32) store32_f32(e.out_f32 + opix * e.out_pitch + e.out_choff + cb, f);
     else if (e.out_hi)
-        store32<kLo, kWide>(e.out_hi + opix * e.out_pitch + e.out_choff + cb,
+        store32<kLo>(e.out_hi + opix * e.out_pitch + e.out_choff + cb,
                      e.out_lo ? e.out_lo + opix * e.out_pitch + e.out_choff + cb : nullptr, f);
     if (tail) {
 #pragma unroll
@@ -181,16 +153,13 @@ __device__ __forceinline__ void epilogue_batch(const ConvParams& p, const float*
     }
 }
 
-// One accumulator row (= one output pixel, all Cout columns) per thread.  `t_addr` = TMEM address of
-// this warp's lane quadrant at the accumulator's first column.  The two warps that share a lane
-// quadrant (chalf 0/1) split the 32-column batches; the conv_12 tail needs a whole row in one
-// thread, so only chalf 0 runs it.  Must be called by all 32 lanes of the warp (tcgen05.ld is
-// warp-collective); chalf is warp-uniform.
-// `nsplit` partial accumulators `split_stride` columns apart (K-split issuers) are summed first.
-constexpr uint32_t kEpiAll = 0xFFFFu, kEpiFp16 = 0x0027u, kEpiSplit = 0x2700u;   // variant masks (bit = variant index)
-template <uint32_t kMask = kEpiAll, bool kSub = false, bool kWide = true>
-__device__ __forceinline__ void epilogue_row(const ConvParams& p, const float* s_par, uint32_t t_addr,
-                                             int n, int oy, int ox, int chalf, int nsplit = 1, int split_stride = 0, int csplit = 2) {
+// One accumulator row (= one output pixel, all Cout columns) per thread, read from the fp32 row `acc` the MMA
+// warpgroups staged in shared memory.  The `csplit` threads that share a row (chalf 0 .. csplit-1) split the 32-column
+// batches; the conv_12 tail needs a whole row in one thread, so only chalf 0 runs it.
+constexpr uint32_t kEpiAll = 0xFFFFu;   // variant mask (bit = variant index)
+template <uint32_t kMask = kEpiAll, bool kSub = false>
+__device__ __forceinline__ void epilogue_row(const ConvParams& p, const float* s_par, const float* acc,
+                                             int n, int oy, int ox, int chalf, int csplit = 2) {
     const EpiParams& e = p.epi;
     const int C = p.Cout;
     const bool pix_ok = oy < p.Hout && ox < p.Wout;
@@ -199,31 +168,25 @@ __device__ __forceinline__ void epilogue_row(const ConvParams& p, const float* s
                              : (static_cast<size_t>(n) * p.Hout + oy) * p.Wout + ox;
     const int ncb = C / 32;
     const bool tail = e.w12 != nullptr;
-    const int cb_first = tail ? 0 : chalf, cb_step = tail ? 1 : csplit;   // csplit warps share a lane quadrant
+    const int cb_first = tail ? 0 : chalf, cb_step = tail ? 1 : csplit;
     const bool active = tail ? (chalf == 0) : (chalf < ncb);
-    if (!active) return;
-    // warp-uniform variant index: activation | second affine | lo plane
+    if (!active || !pix_ok) return;
+    // uniform variant index: activation | second affine | lo plane
     const int variant = e.act | (e.scale2 ? 4 : 0) | ((e.out_lo || e.out2_lo) ? 8 : 0);
     float y3[3] = {0.0f, 0.0f, 0.0f};
     for (int cbi = cb_first; cbi < ncb; cbi += cb_step) {
         const int cb = cbi * 32;
-        uint32_t v[32];
-        __syncwarp();            // lanes of out-of-image pixels skipped the previous batch: reconverge before the warp-collective load
-        tmem_ld32(t_addr + cb, v);
-        tmem_ld_wait();
-        for (int sp = 1; sp < nsplit; ++sp) {
-            uint32_t u[32];
-            tmem_ld32(t_addr + sp * split_stride + cb, u);
-            tmem_ld_wait();
+        float v[32];
 #pragma unroll
-            for (int c = 0; c < 32; ++c) v[c] = __float_as_uint(__uint_as_float(v[c]) + __uint_as_float(u[c]));
+        for (int c = 0; c < 8; ++c) {
+            const float4 a = reinterpret_cast<const float4*>(acc + cb)[c];
+            v[4 * c] = a.x; v[4 * c + 1] = a.y; v[4 * c + 2] = a.z; v[4 * c + 3] = a.w;
         }
-        if (!pix_ok) continue;
         // variants the planner emits (engine.cu build_plan): act 0/1/2, second affine only with ReLU (conv_11_a.2), +8 = lo plane;
         // kMask limits what a kernel instantiates (code size), anything else runs the cold run-time variant
 #define DSU_EPI_CASE(N, A, S2, LO)                                                                                        \
     case N:                                                                                                               \
-        if constexpr ((kMask >> N) & 1u) { epilogue_batch<A, S2, LO, kWide>(p, s_par, v, opix, cb, tail, y3); handled = true; } \
+        if constexpr ((kMask >> N) & 1u) { epilogue_batch<A, S2, LO>(p, s_par, v, opix, cb, tail, y3); handled = true; } \
         break;
         bool handled = false;
         switch (variant) {
@@ -237,10 +200,10 @@ __device__ __forceinline__ void epilogue_row(const ConvParams& p, const float* s
             DSU_EPI_CASE(13, 1, 1, true)
             default: break;
         }
-        if (!handled) epilogue_batch<-1, -1, true, kWide>(p, s_par, v, opix, cb, tail, y3);
+        if (!handled) epilogue_batch<-1, -1, true>(p, s_par, v, opix, cb, tail, y3);
 #undef DSU_EPI_CASE
     }
-    if (tail && pix_ok) {
+    if (tail) {
         const size_t plane = static_cast<size_t>(p.Hout) * p.Wout;
         const size_t pin = static_cast<size_t>(oy) * p.Wout + ox;
         uint8_t rgb[3];

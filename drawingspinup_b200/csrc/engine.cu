@@ -1,7 +1,7 @@
 // Network planner + C ABI (include/dsu_b200.h) of the stylization engine.
 //
 // Turns the constructor arguments of GeneratorJ / GeneratorJ_RIC (training/models.py:24-111,
-// 200-291) and a loaded state dict into a list of fused convolution launches (conv_umma.cu):
+// 200-291) and a loaded state dict into a list of fused convolution launches (conv_wgmma.cu):
 // BatchNorm (eval) is folded into per-channel scale/shift, conv weights are rounded to fp16
 // (hi [+lo]) and pre-swizzled into tensor-core tiles, skip connections / nearest-x2 upsampling /
 // stride / concat become slot tables, and the dead stage-1 smoother conv (models.py:348-350) is
@@ -56,23 +56,12 @@ struct LayerDef {
     int out_buf = -1, out_choff = 0, out_relu = 0, out2_buf = -1;
     int resid_in = 0, resid_out = 0, final = 0;
     int inorm = 0;         // norm_layer='instance_norm': the epilogue leaves the raw fp32 output in a scratch buffer; a type-2 step normalises
-    int halo = 0;          // plain stride-1 conv run by the halo-reuse kernel (conv_halo_persist.cu)
-    int b_bytes = 0;       // bytes of one chunk's weight tile(s) (0 = Cout x 128)
-    int n128 = 0;          // split-fp16 Cout = 64 halo layer packed for the N = 128 issue form (ConvParams::n128)
-    int first = 0;         // one 8-channel group per tap, stride 1: im2col from a shared-memory halo (conv_first.cu)
-    // experimental (DSU_SUBPIXEL=1): sub-pixel class py*2+px of a nearest-x2 + 3x3 convolution (models.py:180-192, SURVEY 8a row a7):
+    // sub-pixel class py*2+px of a nearest-x2 + 3x3 convolution (models.py:180-192, SURVEY 8a row a7):
     // out(2y+py, 2x+px) = sum over a,b in {0,1} of Wc[a][b] * in(y+a-1+py, x+b-1+px), Wc = sums of the 3x3 taps that hit the
     // same source pixel - exact including the zero border, 4 taps instead of 9 per output pixel.  k = 2 for such a layer and
     // wk = 3 is the kernel size of the stored weights; -1 = ordinary layer
     int sub = -1, wk = 0;
-    // tensor-memory RIC kernel (conv_ric_tm.cu): channel runs (one TMA tensor map each), 128-byte blocks, packed weights
-    int tm = 0;
-    struct TmRun { int buf, choff, nch, wch0, wn; };
-    std::vector<TmRun> tm_runs;
-    std::vector<TmBlock> tm_blocks;
-    int tm_nstages = 0;
-    uint8_t* d_wpack_tm = nullptr;
-    CUtensorMap tm_maps[kTmMaxMaps];
+    int first = 0;         // one <= 8-channel segment, stride 1, k > 3 (GeneratorJ.conv0): may run from a shared-memory halo
     // compiled at finalize
     int nchunks = 0, nblocks = 0;
     uint32_t kmask_full = 0xF, kmask_last = 0xF, kmask2_full = 0, kmask2_last = 0;
@@ -89,25 +78,16 @@ struct Step {
 };
 
 // Development knobs: read ONCE from the environment (DSU_<NAME>) by dsu_create, adjustable per handle through
-// dsu_set_knob (tests / tools); 0 = "planner decides" for the sizing knobs.  Defaults are the measured best.
+// dsu_set_knob (tests / tools).
 struct Knobs {
-    int first = 1;            // GeneratorJ.conv0 in the im2col-free kernel (conv_first.cu); 0 = tap mode
-    int first_ks = 0, first_na = 0, first_sets = 0;
-    int halo_persist = 2, halo_ns = 0, halo_ks = 0, halo_na = 0, halo_sb = 0, halo_tps = 0;
+    int first = 1;            // the first layer builds its A chunks from a shared-memory input halo; 0 = tap mode (global loads)
+    int n128 = 1;             // Cout a multiple of 128: N = 128 wgmma instructions; 0 = N = 64 (two instructions per K step)
     int subpixel = 1;         // plan-time: stage-2 nearest-x2 + 3x3 as four 2x2 sub-pixel convolutions
-    int n128 = 2;             // plan-time: split-fp16 Cout = 64 halo layers issue a_hi x [W_hi | W_lo] as one N = 128 MMA: 2 = the 7x7 conv_11 only (measured: 12.8 -> 11.0 ms; the 3x3 smoothers lose 10-30 % without their second accumulator set), 1 = all, 0 = off
-    int halo_nsets = 0;       // 1 = force a single accumulator set in the persistent halo kernel (measurements)
-    int tm_ni = 0, tm_sb = 0; // tensor-memory kernel: issuing warps / weight stages (0 = planner decides)
     int derive_edge = 0;      // stage 2, no edge map passed: burn the edges pos2edge finds in the pos frames (fused into the ingest)
-    int tm_trace = 0;         // development: 1 + index of the launch step whose CTA 0 records an event trace (dsu_debug_watchdog slots 32..)
 };
 struct KnobName { const char* name; int Knobs::*field; };
 const KnobName kKnobNames[] = {
-    {"first", &Knobs::first}, {"first_ks", &Knobs::first_ks}, {"first_na", &Knobs::first_na},
-    {"first_sets", &Knobs::first_sets}, {"halo_persist", &Knobs::halo_persist}, {"halo_ns", &Knobs::halo_ns},
-    {"halo_ks", &Knobs::halo_ks}, {"halo_na", &Knobs::halo_na}, {"halo_sb", &Knobs::halo_sb}, {"halo_tps", &Knobs::halo_tps},
-    {"subpixel", &Knobs::subpixel}, {"tm_ni", &Knobs::tm_ni}, {"tm_sb", &Knobs::tm_sb}, {"tm_trace", &Knobs::tm_trace}, {"derive_edge", &Knobs::derive_edge},
-    {"n128", &Knobs::n128}, {"halo_nsets", &Knobs::halo_nsets},
+    {"first", &Knobs::first}, {"n128", &Knobs::n128}, {"subpixel", &Knobs::subpixel}, {"derive_edge", &Knobs::derive_edge},
 };
 Knobs knobs_from_env() {
     Knobs k;
@@ -155,11 +135,7 @@ struct dsu_engine {
     std::set<std::string> loaded;
     std::vector<LayerDef> layers;
     std::vector<Step> steps;
-    unsigned long long* wd_host = nullptr;   // watchdog records of the tensor-memory kernel (pinned, device-mapped)
-    unsigned long long* wd_dev = nullptr;
-    bool ric_tm = false;      // stage 1 on the tensor-memory kernel
-    bool f32_acts = false;    // ... and (split-fp16 mode) its activation buffers hold fp32 instead of fp16 hi + lo planes
-    int maps_B = 0, maps_H = 0, maps_W = 0;
+    bool f32_acts = false;    // stage 1 in split-fp16 mode: activation buffers hold fp32 instead of fp16 hi + lo planes
     int buf_level[NBUF]{}, buf_C[NBUF]{};
     bool buf_used[NBUF]{};
     float *d_w12 = nullptr, *d_b12 = nullptr;
@@ -289,7 +265,7 @@ int build_plan(dsu_engine* E) {
         add(Bl);
     }
     // plain (stage-2) up-convolutions run as four sub-pixel 2x2 convolutions on the low-resolution source (2.25x fewer
-    // MACs; validated on hardware in round 2, profiles/r02a_experimental.log); DSU_SUBPIXEL=0 at dsu_create restores the 3x3 form
+    // MACs); DSU_SUBPIXEL=0 at dsu_create restores the 3x3 form
     const bool subpixel = !ric && E->knobs.subpixel != 0;
     auto add_up = [&](LayerDef L) {
         L.inorm = inorm;
@@ -335,7 +311,6 @@ int build_plan(dsu_engine* E) {
         L.segs = {{ric ? C11 : S0, 0, f[5], 0, f[5]}}; L.act = 1; L.final = 1;
         add(L);
     }
-    for (LayerDef& L : E->layers) L.tm = L.ric ? 1 : 0;       // every stage-1 convolution runs the tensor-memory RIC kernel
     return DSU_OK;
 }
 
@@ -347,70 +322,6 @@ int upload(T** dst, const std::vector<T>& src) {
     CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(dst), src.size() * sizeof(T)));
     CUDA_TRY(cudaMemcpy(*dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice));
     return DSU_OK;
-}
-
-// Tensor-memory RIC kernel (conv_ric_tm.cu): channel runs -> 128-byte blocks -> stages, and the weights as
-// [stage][tap][part][Cout x 32 B] no-swizzle K-major tiles (8-row x 16-byte core matrices: element (o, c) of a 16-channel
-// K step at (o / 8) * 256 + (c / 8) * 128 + (o % 8) * 16 + (c % 8) * 2; descriptor LBO = 128, SBO = 256 - tools/umma_ts_probe.cu).
-// fp16 mode: a stage = 32 channels = two K16 steps (part = step).  split-fp16: a stage = 16 fp32 channels = one K16 step,
-// part 0 = W_hi, part 1 = W_lo = fp16(W - W_hi).
-int compile_tm(dsu_engine* E, LayerDef& L, const std::vector<float>& Wt, int cin_total) {
-    const bool exact = E->exact;
-    const int C = L.cout, k = L.k;
-    if (k != 3 || L.stride != 1) return fail(DSU_E_INVALID, "tensor-memory RIC kernel: 3x3 stride-1 layers only: " + L.name);
-    // consecutive segments that continue each other in the same buffer AND in the weight's input channels form one run
-    L.tm_runs.clear();
-    for (const SegDef& sg : L.segs) {
-        if (!L.tm_runs.empty()) {
-            LayerDef::TmRun& r = L.tm_runs.back();
-            if (r.buf == sg.buf && r.choff + r.nch == sg.choff && r.wch0 + r.nch == sg.wch0 && r.wn == r.nch) {
-                r.nch += sg.nch; r.wn += sg.wn;
-                continue;
-            }
-        }
-        L.tm_runs.push_back(LayerDef::TmRun{sg.buf, sg.choff, sg.nch, sg.wch0, sg.wn});
-    }
-    if (L.tm_runs.size() > kTmMaxMaps) return fail(DSU_E_INVALID, "tensor-memory RIC kernel: too many concat runs: " + L.name);
-    const int bs = exact ? 32 : 64, ss = bs / 2, chunk_ch = exact ? 4 : 8;     // channels per block / stage / 16-byte chunk
-    L.tm_blocks.clear();
-    struct StageSrc { int run, c0; };          // first run channel of the stage
-    std::vector<StageSrc> stages;
-    for (size_t ri = 0; ri < L.tm_runs.size(); ++ri) {
-        const LayerDef::TmRun& r = L.tm_runs[ri];
-        for (int c0 = 0; c0 < r.nch; c0 += bs) {
-            const int nch = std::min(bs, r.nch - c0);
-            TmBlock b{};
-            b.map = static_cast<uint8_t>(ri);
-            b.c0 = static_cast<uint16_t>(c0);
-            b.nstages = static_cast<uint8_t>(nch > ss ? 2 : 1);
-            for (int h = 0; h < b.nstages; ++h) {
-                b.chunks[h] = static_cast<uint8_t>((std::min(ss, nch - h * ss) + chunk_ch - 1) / chunk_ch);
-                stages.push_back(StageSrc{static_cast<int>(ri), c0 + h * ss});
-            }
-            L.tm_blocks.push_back(b);
-        }
-    }
-    if (L.tm_blocks.size() > kTmMaxBlocks) return fail(DSU_E_INVALID, "tensor-memory RIC kernel: too many channel blocks: " + L.name);
-    L.tm_nstages = static_cast<int>(stages.size());
-    const size_t tile = static_cast<size_t>(C) * 32, stage_bytes = tile * 18;
-    std::vector<uint8_t> pack(stages.size() * stage_bytes, 0);
-    for (size_t si = 0; si < stages.size(); ++si) {
-        const LayerDef::TmRun& r = L.tm_runs[stages[si].run];
-        for (int t = 0; t < 9; ++t)
-            for (int part = 0; part < 2; ++part) {
-                uint8_t* dst = pack.data() + si * stage_bytes + (static_cast<size_t>(t) * 2 + part) * tile;
-                for (int o = 0; o < C; ++o)
-                    for (int c = 0; c < 16; ++c) {
-                        const int rc = stages[si].c0 + (exact ? c : 16 * part + c);      // channel inside the run
-                        if (rc >= r.wn) continue;                                          // K padding: zero weight
-                        const float wv = Wt[((static_cast<size_t>(o) * cin_total + r.wch0 + rc) * 3 + t / 3) * 3 + t % 3];
-                        const __half wh = __float2half_rn(wv);
-                        const __half val = (exact && part == 1) ? __float2half_rn(wv - __half2float(wh)) : wh;
-                        std::memcpy(dst + (o / 8) * 256 + (c / 8) * 128 + (o % 8) * 16 + (c % 8) * 2, &val, 2);
-                    }
-            }
-    }
-    return upload(&L.d_wpack_tm, pack);
 }
 
 int compile_layer(dsu_engine* E, LayerDef& L) {
@@ -447,13 +358,6 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     const std::vector<float>& Wt = L.sub >= 0 ? Wsub : E->w.at(L.wkey);
     if (Wt.size() != static_cast<size_t>(C) * cin_total * k * k) return fail(DSU_E_INVALID, "weight size mismatch for " + L.wkey);
 
-    double real_k_tm = 0;
-    for (const SegDef& sg : L.segs) real_k_tm += static_cast<double>(sg.wn) * k * k;
-    if (L.tm) {
-        L.macs_per_px = real_k_tm * C;
-        int rc_tm = compile_tm(E, L, Wt, cin_total);
-        if (rc_tm) return rc_tm;
-    } else {
     // A "data slot" is 8 input channels of one concat segment at one tap.  A chunk (8 smem slots =
     // 64 K elements) holds 8 data slots (fp16 mode) or 4 data slots as [hi x4 | lo x4] (exact mode).
     // plain conv: data slots are packed densely over (tap, segment, channel group);
@@ -467,10 +371,12 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     L.macs_per_px = real_k * C;
     // algorithmic work of a sub-pixel class = a quarter of the 3x3 layer's output pixels (flops are reported per output pixel of level_out)
     if (L.sub >= 0) L.macs_per_px = real_k / 4.0 * 9.0 / 4.0 * C;
+    // a sub-pixel class (py, px) pads its 2x2 window by (1 - py, 1 - px) above and left
+    const int pad_y = L.sub >= 0 ? 1 - (L.sub >> 1) : L.pad, pad_x = L.sub >= 0 ? 1 - (L.sub & 1) : L.pad;
     auto dev_slot = [&](const HSlot& h, bool lo_plane) {
         Slot sl{};
-        sl.dy = static_cast<int8_t>(h.kh - L.pad);
-        sl.dx = static_cast<int8_t>(h.kw - L.pad);
+        sl.dy = static_cast<int8_t>(h.kh - pad_y);
+        sl.dx = static_cast<int8_t>(h.kw - pad_x);
         sl.seg = static_cast<uint8_t>(h.seg + (lo_plane ? kMaxSeg / 2 : 0));
         sl.valid = 1;
         sl.choff = static_cast<uint16_t>(h.choff);
@@ -483,18 +389,8 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
             else slots.push_back(Slot{});
         }
     };
-    // halo-reuse kernel: plain stride-1 convs with >= 32 channels per tap (the 8-channel 7x7 conv0 was measured slower
-    // there: 49 single-K-step MMAs per tile; it has its own kernel, conv_first.cu, and the tap-mode kernel as fallback)
-    L.halo = (!L.ric && L.stride == 1 && real_k / (k * k) >= 32) ? 1 : 0;
-    // split-fp16, Cout = 64: [W_hi ; W_lo] x 32-channel no-swizzle tiles, a_hi x [W_hi | W_lo] as one N = 128 MMA (ConvParams::n128)
-    L.n128 = (L.halo && exact && C == 64 && (E->knobs.n128 == 1 || (E->knobs.n128 == 2 && k > 3))) ? 1 : 0;
-    if (!L.ric && !L.halo) {
-        // single 8-channel group per tap (conv0 of GeneratorJ), fp16 mode: one chunk per KERNEL ROW (slot j = tap (kh, j)),
-        // the layout the im2col-free kernel (conv_first.cu) needs; the tap-mode kernel runs the same table
-        // split-fp16: the same kernel with a second (lo) halo plane and [W_hi ; W_lo] tile pairs per kernel row - a layout the
-        // tap-mode kernel cannot run, so there the choice is made here (knob `first`, plan-time) and not per launch
-        L.first = ((!exact || E->knobs.first != 0) && L.stride == 1 && L.up == 0 && L.segs.size() == 1 && L.segs[0].nch <= 8 && k > 3 &&
-                   k <= 8 && L.pad == (k - 1) / 2) ? 1 : 0;
+    if (!L.ric) {
+        L.first = (L.stride == 1 && L.up == 0 && L.sub < 0 && L.segs.size() == 1 && L.segs[0].nch <= 8 && k > 3 && L.pad == (k - 1) / 2) ? 1 : 0;
         std::vector<HSlot> all;
         for (int kh = 0; kh < k; ++kh) {
             for (int kw = 0; kw < k; ++kw)
@@ -503,11 +399,6 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
                     for (int c8 = 0; c8 < s.nch; c8 += 8)
                         all.push_back(HSlot{kh, kw, (int)si, s.choff + c8, s.wch0 + c8, std::max(0, std::min(8, s.wn - c8))});
                 }
-            if (L.first) {
-                push_dev_slots(all);
-                chunks.push_back(all);
-                all.clear();
-            }
         }
         for (size_t i = 0; i < all.size(); i += dpc) {
             std::vector<HSlot> ds(all.begin() + i, all.begin() + std::min(all.size(), i + dpc));
@@ -535,9 +426,7 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     }
     L.nchunks = static_cast<int>(chunks.size());
     std::vector<ChunkHdr> hdrs(L.nchunks);
-    const bool first_exact = L.first && exact;      // chunk = kernel row: a W_hi tile followed by a W_lo tile (8 tap slots each)
-    const size_t tile = static_cast<size_t>(C) * 128 * (first_exact ? 2 : 1);
-    L.b_bytes = static_cast<int>(tile);
+    const size_t tile = static_cast<size_t>(C) * 128;
     std::vector<uint8_t> pack(static_cast<size_t>(L.nchunks) * tile, 0);
     size_t off = 0;
     auto put = [&](size_t tile_off, int row, int slot, int ci, __half val) {
@@ -549,9 +438,7 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
         const int nd = static_cast<int>(ds.size());
         const int steps = (nd + 1) / 2;                        // K=16 steps covering the data slots
         ChunkHdr& hd = hdrs[q];
-        hd.pad_ = 0;
-        hd.b_off = static_cast<uint32_t>(off);
-        if (!exact || L.n128 || first_exact) { hd.kmask = static_cast<uint8_t>((1 << steps) - 1); hd.kmask2 = 0; }
+        if (!exact) { hd.kmask = static_cast<uint8_t>((1 << steps) - 1); hd.kmask2 = 0; }
         else { hd.kmask = static_cast<uint8_t>(((1 << steps) - 1) | (((1 << steps) - 1) << 2)); hd.kmask2 = static_cast<uint8_t>((1 << steps) - 1); }
         // B tile(s): row o = output channel, 128 B = 64 K elements, 16-byte slots XOR-swizzled by (row & 7)
         for (int o = 0; o < C; ++o)
@@ -560,18 +447,8 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
                 for (int ci = 0; ci < h.nvalid; ++ci) {
                     const float wv = Wt[((static_cast<size_t>(o) * cin_total + h.wch + ci) * k + h.kh) * k + h.kw];
                     const __half wh = __float2half_rn(wv);
-                    if (L.n128) {
-                        // no-swizzle K-major tile of 128 rows x 32 channels: rows 0-63 W_hi, 64-127 W_lo; 8 x 16 B core matrices,
-                        // K-adjacent core matrices 128 B apart, 8-row groups 512 B apart
-                        const __half wl = __float2half_rn(wv - __half2float(wh));
-                        auto at = [&](int row) { return off + static_cast<size_t>(row / 8) * 512 + static_cast<size_t>(d) * 128 + (row % 8) * 16 + ci * 2; };
-                        std::memcpy(&pack[at(o)], &wh, 2);
-                        std::memcpy(&pack[at(o + 64)], &wl, 2);
-                        continue;
-                    }
                     put(off, o, d, ci, wh);
-                    if (first_exact) put(off + static_cast<size_t>(C) * 128, o, d, ci, __float2half_rn(wv - __half2float(wh)));
-                    else if (exact) put(off, o, d + 4, ci, __float2half_rn(wv - __half2float(wh)));   // [W_hi | W_lo] in one row
+                    if (exact) put(off, o, d + 4, ci, __float2half_rn(wv - __half2float(wh)));   // [W_hi | W_lo] in one row
                 }
             }
         off += tile;
@@ -582,7 +459,6 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     int rc_up;
     if ((rc_up = upload(&L.d_slots, slots))) return rc_up;
     if ((rc_up = upload(&L.d_wpack, pack))) return rc_up;
-    }
     int rc;
 
     // epilogue affine: y = act(acc * scale + shift) [* scale2 + shift2]
@@ -701,45 +577,6 @@ int build_level(dsu_engine* E, Level& lv, int h, int w) {
     return DSU_OK;
 }
 
-// ------------------------------------------------------------------ TMA tensor maps of the tensor-memory RIC layers
-// One 4-D map (channel, x, y, frame) per channel run of a layer's input concat: base = first channel of the run, extent =
-// the run's channels, so that everything outside the run / the image reads as zero.  Box = 128 bytes of channels x the halo
-// tile of an 8 x 16 output tile (18 x 10 pixels; 10 x 6 source pixels when the layer's nearest x2 is folded in), SWIZZLE_128B.
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-int build_tensor_maps(dsu_engine* E, int B, int H, int W) {
-    static EncodeTiledFn encode = nullptr;
-    if (!encode) {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        CUDA_TRY(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-        if (!fn || qres != cudaDriverEntryPointSuccess) return fail(DSU_E_CUDA, "cuTensorMapEncodeTiled is not available in this driver");
-        encode = reinterpret_cast<EncodeTiledFn>(fn);
-    }
-    const size_t esz = E->f32_acts ? sizeof(float) : sizeof(__half);
-    for (LayerDef& L : E->layers) {
-        if (!L.tm) continue;
-        for (size_t ri = 0; ri < L.tm_runs.size(); ++ri) {
-            const LayerDef::TmRun& r = L.tm_runs[ri];
-            const int lvl = E->buf_level[r.buf];
-            const cuuint64_t hs = static_cast<cuuint64_t>(H >> lvl), ws = static_cast<cuuint64_t>(W >> lvl);
-            const cuuint64_t pitch_b = static_cast<cuuint64_t>(E->buf_C[r.buf]) * esz;
-            const cuuint64_t dims[4] = {static_cast<cuuint64_t>(r.nch), ws, hs, static_cast<cuuint64_t>(B)};
-            const cuuint64_t strides[3] = {pitch_b, pitch_b * ws, pitch_b * ws * hs};
-            const cuuint32_t box[4] = {static_cast<cuuint32_t>(128 / esz), L.up ? 10u : 18u, L.up ? 6u : 10u, 1u};
-            const cuuint32_t estr[4] = {1, 1, 1, 1};
-            void* basep = reinterpret_cast<uint8_t*>(E->buf_hi[r.buf]) + static_cast<size_t>(r.choff) * esz;
-            const CUresult cr = encode(&L.tm_maps[ri], E->f32_acts ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, basep,
-                                       dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                       CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (cr != CUDA_SUCCESS)
-                return fail(DSU_E_CUDA, "cuTensorMapEncodeTiled failed (" + std::to_string(static_cast<int>(cr)) + ") for " + L.name);
-        }
-    }
-    return DSU_OK;
-}
-
 // ------------------------------------------------------------------ workspace
 int ensure_shape(dsu_engine* E, int B, int H, int W) {
     if (B <= 0 || H <= 0 || W <= 0 || (H % 4) || (W % 4))
@@ -753,7 +590,6 @@ int ensure_shape(dsu_engine* E, int B, int H, int W) {
             if (E->buf_hi[b]) cudaFree(E->buf_hi[b]);
             if (E->buf_lo[b]) cudaFree(E->buf_lo[b]);
             E->buf_hi[b] = E->buf_lo[b] = nullptr;
-            E->maps_B = 0;                                   // tensor maps point into the old allocation
             CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->buf_hi[b]), bytes));
             CUDA_TRY(cudaMemset(E->buf_hi[b], 0, bytes));
             if (E->exact && !E->f32_acts) {
@@ -798,28 +634,12 @@ int ensure_shape(dsu_engine* E, int B, int H, int W) {
             if (rc) return rc;
         }
     E->B = B; E->H = H; E->W = W;
-    if (E->cfg.kind == DSU_KIND_GENERATORJ_RIC && (E->maps_B != B || E->maps_H != H || E->maps_W != W)) {
-        int rc = build_tensor_maps(E, B, H, W);
-        if (rc) return rc;
-        E->maps_B = B; E->maps_H = H; E->maps_W = W;
-    }
     return DSU_OK;
-}
-
-// stage counts of the tap-mode kernel: one ring depth for A and B, aiming at two CTAs per SM
-void pick_stages(int b_bytes, int* sa, int* sb) {
-    const int stage = kABytes + b_bytes;
-    int s = (108 * 1024) / stage;
-    if (s < 2) s = (216 * 1024) / stage;
-    s = std::max(2, std::min(kMaxStagesB, s));
-    *sa = s; *sb = s;
 }
 
 int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgba, const uint8_t* alpha_src,
                 int alpha_stride, cudaStream_t st, std::vector<cudaEvent_t>* evs = nullptr) {
     size_t step_idx = 0;
-    const Knobs& K = E->knobs;
-    const int first_mode = K.first;
     for (const Step& sp : E->steps) {
         if (evs) CUDA_TRY(cudaEventRecord((*evs)[step_idx], st));
         ++step_idx;
@@ -863,13 +683,11 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
         p.up = L.up; p.Hv = p.Hin << L.up; p.Wv = p.Win << L.up;
         p.stride = L.stride; p.ric = L.ric; p.exact = E->exact ? 1 : 0;
         p.nchunks = L.nchunks; p.nblocks = L.nblocks; p.Cout = L.cout;
-        p.b_bytes = L.b_bytes > 0 ? L.b_bytes : L.cout * 128;
+        p.b_bytes = L.cout * 128;
         p.kmask_full = L.kmask_full; p.kmask_last = L.kmask_last; p.kmask2_full = L.kmask2_full; p.kmask2_last = L.kmask2_last;
-        pick_stages(p.b_bytes, &p.sa, &p.sb);
-        p.ks = 1;
-        int cols = 32;
-        while (cols < p.ks * L.cout) cols *= 2;
-        p.tmem_cols = cols;
+        if (L.sub >= 0) { p.sub = 1; p.sub_py = L.sub >> 1; p.sub_px = L.sub & 1; }
+        p.halo = L.first && E->knobs.first != 0; p.ksize = L.k; p.pad = L.pad;
+        p.n128 = E->knobs.n128 != 0;
         p.slots = L.d_slots; p.wpack = L.d_wpack;
         for (size_t i = 0; i < L.segs.size(); ++i) {
             p.seg[i].ptr = E->buf_hi[L.segs[i].buf];
@@ -900,129 +718,7 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
             e.w12 = E->d_w12; e.b12 = E->d_b12; e.tanh_flag = E->cfg.tanh;
             e.y_nchw = y_dev; e.y_rgba = y_rgba; e.alpha_src = alpha_src; e.alpha_stride = alpha_stride;
         }
-        if (L.tm) {
-            // tensor-memory RIC kernel: accumulator sets / A stages share the 512 TMEM columns, weight stages fill shared memory
-            TmParams T{};
-            T.c = p;
-            for (size_t i = 0; i < L.tm_runs.size(); ++i) T.tmap[i] = L.tm_maps[i];
-            T.nblocks = static_cast<int>(L.tm_blocks.size());
-            for (int i = 0; i < T.nblocks; ++i) T.blk[i] = L.tm_blocks[i];
-            T.nstages = L.tm_nstages;
-            T.sa = 2;
-            T.nsets = (2 * L.cout + T.sa * kTmStageCols <= 512) ? 2 : 1;
-            T.b_stage_bytes = L.cout * 576;
-            int sb = static_cast<int>((227 * 1024 - 2 * kTmHaloBytes - 8 * 1024) / T.b_stage_bytes);
-            sb = std::min(sb, 6);
-            if (K.tm_sb > 0) sb = std::min(sb, K.tm_sb);
-            sb = (sb / T.sa) * T.sa;
-            if (sb < T.sa) return fail(DSU_E_INVALID, "tensor-memory RIC kernel: the weight stages do not fit in shared memory: " + L.name);
-            T.sb = sb;
-            T.ni = K.tm_ni > 0 ? std::min(K.tm_ni, kTmIssuerWarps) : kTmIssuerWarps;
-            T.halo_w = L.up ? 10 : 18; T.halo_h = L.up ? 6 : 10;
-            T.wpack = L.d_wpack_tm;
-            if (!E->wd_host) {
-                if (cudaHostAlloc(reinterpret_cast<void**>(&E->wd_host), (32 + 5 * 1024) * sizeof(unsigned long long), cudaHostAllocMapped) == cudaSuccess) {
-                    std::memset(E->wd_host, 0, (32 + 5 * 1024) * sizeof(unsigned long long));
-                    if (cudaHostGetDevicePointer(reinterpret_cast<void**>(&E->wd_dev), E->wd_host, 0) != cudaSuccess) E->wd_dev = nullptr;
-                } else {
-                    E->wd_host = nullptr;
-                    (void)cudaGetLastError();
-                }
-            }
-            T.dbg = E->wd_dev;
-            T.trace = (E->wd_dev && K.tm_trace > 0 && static_cast<size_t>(K.tm_trace) == step_idx) ? E->wd_dev + 32 : nullptr;
-            CUDA_TRY(launch_conv_ric_tm(T, st));
-            continue;
-        }
-        if (L.halo) {
-            // ns sub-tiles x ks K-split issuers (<= 4 issuing warps, <= 512 TMEM columns); shared memory:
-            // 2 halo buffers + as many weight stages as fit
-            const int kk = L.k, pp = L.pad;
-            p.halo = 1; p.ksize = kk; p.pad = pp;
-            if (L.sub >= 0) {
-                p.sub = 1; p.sub_py = L.sub >> 1; p.sub_px = L.sub & 1;
-                p.pad_y = 1 - p.sub_py; p.pad_x = 1 - p.sub_px;
-            }
-            const int halo_extra = L.sub >= 0 ? kk - 1 : 2 * pp;     // halo pixels beyond the output tile, per axis
-            // candidates in order of measured preference (profiles/r01d sweep): wide CTAs for 3x3 (weight-tile reuse),
-            // sub-tile x K-split for 7x7 (halo size); the first that fits TMEM and shared memory wins
-            // {sub-tiles, K-split issuers, halo buffers}
-            static const int cand3[][3] = {{4, 1, 2}, {2, 2, 2}, {2, 1, 2}, {1, 2, 2}, {1, 1, 2}};
-            static const int cand7[][3] = {{4, 1, 1}, {2, 2, 2}, {2, 1, 2}, {1, 2, 2}, {1, 1, 2}};
-            static const int cand3n[][3] = {{2, 1, 2}, {4, 1, 2}, {1, 1, 2}, {1, 1, 2}, {1, 1, 2}};   // n128 form: two accumulator sets first
-            const int (*cand)[3] = kk <= 3 ? (L.n128 ? cand3n : cand3) : cand7;
-            const int persist_mode = K.halo_persist;   // 0 never, 1 when the chosen config allows, 2 prefer (measured best)
-            const int env_ns = K.halo_ns > 0 ? std::min(4, K.halo_ns) : 0, env_ks = K.halo_ks > 0 ? std::min(4, K.halo_ks) : 0;
-            const int env_na = K.halo_na > 0 ? std::min(3, K.halo_na) : 0;
-            bool found = false;
-            const int acw = L.n128 ? 2 : 1;             // accumulator width per issuer in units of Cout
-            p.n128 = L.n128;
-            for (int ci = 0; ci < 5 && !found; ++ci) {
-                const int ns = env_ns ? env_ns : cand[ci][0], ks = L.n128 ? 1 : (env_ks ? env_ks : cand[ci][1]);
-                if (ns * ks > kIssuersHalo || ns * ks * acw * L.cout > 512 || ks > kk * kk) continue;
-                // only configurations that can double-buffer TMEM (the n128 form may run with a single accumulator set)
-                if (persist_mode == 2 && !L.n128 && 2 * ns * ks * L.cout > 512) continue;
-                p.ns = ns; p.ks = ks;
-                p.halo_w = 8 * ns + halo_extra;
-                p.halo_rows = (16 + halo_extra) * p.halo_w;
-                p.halo_bytes = (p.halo_rows * 128 + 1023) & ~1023;
-                p.sa = env_na ? env_na : cand[ci][2];
-                const int left = 227 * 1024 - p.sa * p.halo_bytes - 8 * 1024;
-                p.sb = left < 0 ? 0 : std::min(kMaxStagesB, left / p.b_bytes);
-                if (K.halo_sb > 0) p.sb = std::max(2, std::min(p.sb, K.halo_sb));
-                p.sb = (p.sb / ks) * ks;
-                found = p.sb / ks >= 3 || (ci == 4 && p.sb / ks >= 2);
-            }
-            if (!found) return fail(DSU_E_INVALID, "halo convolution does not fit in shared memory: " + L.name);
-            // persistent CTAs with double-buffered accumulators when two accumulator sets fit in TMEM
-            p.nsets = 2 * p.ns * p.ks * acw * L.cout <= 512 ? 2 : 1;
-            if (K.halo_nsets == 1) p.nsets = 1;
-            const bool persist = persist_mode != 0;      // the persistent kernel runs with one accumulator set when two do not fit
-            p.tps = 1;
-            if (persist) {   // taps per weight stage: up to 3 while the ring stays >= 3 stages deep (per K-split group)
-                int tps = 3;
-                if (K.halo_tps > 0) tps = std::max(1, std::min(4, K.halo_tps));
-                const int left = 227 * 1024 - p.sa * p.halo_bytes - 8 * 1024;
-                while (tps > 1 && (left / (tps * p.b_bytes)) / p.ks < 3) --tps;
-                p.tps = tps;
-                p.sb = std::min(kMaxStagesB, left / (tps * p.b_bytes));
-                p.sb = (p.sb / p.ks) * p.ks;
-            }
-            cols = 32;
-            while (cols < p.nsets * p.ns * p.ks * acw * L.cout) cols *= 2;
-            p.tmem_cols = cols;
-            if (!persist) return fail(DSU_E_INVALID, "halo convolution: the non-persistent kernel was removed (knob halo_persist = 0): " + L.name);
-            CUDA_TRY(launch_conv_halo_persist(p, st));
-        } else {
-            bool first = false;
-            if (L.first && (first_mode != 0 || E->exact)) {
-                // im2col-free persistent kernel: ring of pixel-linear halo tiles + the whole weight matrix in shared memory
-                p.ksize = L.k; p.pad = L.pad;
-                p.halo_w = 16;
-                p.halo_rows = 16 + L.k - 1;
-                p.halo_bytes = p.halo_rows * 16 * 16 * (E->exact ? 2 : 1);      // split-fp16: hi plane, then lo plane
-                const int ks_max = std::min(4, std::min(L.k, 256 / L.cout));
-                p.ks = std::min(2, ks_max);
-                if (K.first_ks > 0) p.ks = std::max(1, std::min(ks_max, K.first_ks));
-                const int left = 227 * 1024 - L.nchunks * p.b_bytes - 8 * 1024;
-                p.sa = std::min(4, left / p.halo_bytes);
-                if (K.first_na > 0) p.sa = std::max(2, std::min(6, std::min(left / p.halo_bytes, K.first_na)));
-                if (p.ks >= 1 && p.sa >= 2) {
-                    p.ns = 4 * p.ks * L.cout <= 512 ? 4 : 2;          // accumulator sets in TMEM
-                    if (K.first_sets > 0) p.ns = (K.first_sets >= 4 && p.ns == 4) ? 4 : 2;
-                    cols = 32;
-                    while (cols < p.ns * p.ks * L.cout) cols *= 2;
-                    p.tmem_cols = cols;
-                    first = true;
-                }
-            }
-            if (first) CUDA_TRY(launch_conv_first(p, st));
-            else {
-                pick_stages(p.b_bytes, &p.sa, &p.sb);
-                p.ks = 1;
-                CUDA_TRY(launch_conv(p, st));
-            }
-        }
+        CUDA_TRY(launch_conv(p, st));
     }
     if (evs) CUDA_TRY(cudaEventRecord((*evs)[step_idx], st));
     return DSU_OK;
@@ -1040,7 +736,7 @@ int check_ready(dsu_handle h) {
 extern "C" {
 
 const char* dsu_last_error(void) { return g_err.c_str(); }
-const char* dsu_version(void) { return "dsu_b200 0.1 (sm_100a, tcgen05)"; }
+const char* dsu_version(void) { return "dsu_b200 0.2 (sm_90a, wgmma)"; }
 
 int dsu_create(const dsu_config* cfg, dsu_handle* out) {
     if (!cfg || !out) return fail(DSU_E_INVALID, "null argument");
@@ -1062,21 +758,14 @@ int dsu_create(const dsu_config* cfg, dsu_handle* out) {
     if (cfg->device < 0 || cfg->device >= ndev) return fail(DSU_E_INVALID, "no such CUDA device");
     cudaDeviceProp prop{};
     CUDA_TRY(cudaGetDeviceProperties(&prop, cfg->device));
-    if (prop.major != 10)
-        return fail(DSU_E_INVALID, std::string("device '") + prop.name + "' is not sm_100 (tcgen05 kernels only, no fallback path)");
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(DSU_E_INVALID, std::string("device '") + prop.name + "' is not sm_90 (wgmma kernels built for sm_90a only, no fallback path)");
     dsu_engine* E = new dsu_engine();
     E->cfg = *cfg;
     E->knobs = knobs_from_env();
-    // stage 1 runs the tensor-memory RIC kernel: accumulator + two A stages must fit the 512 TMEM columns
-    E->ric_tm = cfg->kind == DSU_KIND_GENERATORJ_RIC;
-    for (int i = 0; i < 6; ++i)
-        if (E->ric_tm && cfg->filters[i] > 224) {
-            delete E;
-            return fail(DSU_E_INVALID, "GeneratorJ_RIC: filters must be <= 224 (tensor-memory budget of the RIC kernel)");
-        }
     E->cin_pad = (cfg->input_channels + 7) / 8 * 8;
     E->exact = cfg->precision == DSU_PREC_FP16X3;
-    E->f32_acts = E->ric_tm && E->exact;
+    E->f32_acts = cfg->kind == DSU_KIND_GENERATORJ_RIC && E->exact;
     int rc = build_plan(E);
     if (rc) { delete E; return rc; }
     *out = E;
@@ -1087,14 +776,13 @@ void dsu_destroy(dsu_handle h) {
     if (!h) return;
     DeviceGuard guard(h->cfg.device);
     for (LayerDef& L : h->layers) {
-        cudaFree(L.d_slots); cudaFree(L.d_wpack); cudaFree(L.d_wpack_tm);
+        cudaFree(L.d_slots); cudaFree(L.d_wpack);
         cudaFree(L.d_scale); cudaFree(L.d_shift); cudaFree(L.d_scale2); cudaFree(L.d_shift2);
     }
     for (int b = 0; b < NBUF; ++b) { cudaFree(h->buf_hi[b]); cudaFree(h->buf_lo[b]); }
     for (int l = 0; l < 3; ++l) { cudaFree(h->lv[l].lyx); cudaFree(h->lv[l].oct); cudaFree(h->lv[l].wh); }
     cudaFree(h->resid); cudaFree(h->d_w12); cudaFree(h->d_b12);
     cudaFree(h->inorm_x); cudaFree(h->inorm_stats); cudaFree(h->inorm_acc);
-    if (h->wd_host) cudaFreeHost(h->wd_host);
     cudaFree(h->io_color); cudaFree(h->io_pos); cudaFree(h->io_edge); cudaFree(h->io_out);
     delete h;
 }
@@ -1151,8 +839,6 @@ int dsu_set_knob(dsu_handle h, const char* name, int32_t value) {
         if (std::strcmp(kn.name, name) == 0) {
             if (kn.field == &Knobs::subpixel && h->knobs.subpixel != value)
                 return fail(DSU_E_STATE, "'subpixel' shapes the launch plan: set DSU_SUBPIXEL in the environment before dsu_create");
-            if (kn.field == &Knobs::n128 && h->knobs.n128 != value)
-                return fail(DSU_E_STATE, "'n128' shapes the weight packing: set DSU_N128 in the environment before dsu_create");
             h->knobs.*(kn.field) = value;
             return DSU_OK;
         }
@@ -1336,16 +1022,6 @@ int dsu_pos2edge(const uint8_t* pos_dev, int32_t B, int32_t H, int32_t W, uint8_
     if (!pos_dev || !edge_dev || B <= 0 || H <= 0 || W <= 0) return fail(DSU_E_INVALID, "bad argument");
     CUDA_TRY(pos2edge(pos_dev, B, H, W, edge_dev, static_cast<cudaStream_t>(stream)));
     return DSU_OK;
-}
-
-int dsu_debug_watchdog(dsu_handle h, uint64_t* out, int32_t n) {
-    if (!h || !out) return fail(DSU_E_INVALID, "null argument");
-    int found = 0;
-    for (int i = 0; i < n; ++i) {
-        out[i] = (h->wd_host && i < 32 + 5 * 1024) ? h->wd_host[i] : 0;
-        if (out[i]) ++found;
-    }
-    return found;
 }
 
 int dsu_debug_read(dsu_handle h, int32_t buffer, int32_t plane, void* dst_host, size_t bytes) {

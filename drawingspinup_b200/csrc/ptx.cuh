@@ -1,6 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the conv kernels use:
-// mbarrier, 1-D bulk async copy, cp.async, tcgen05 (alloc / mma / commit / ld), proxy fences.
-// sm_100a only - there is no fallback path.
+// Thin inline-PTX wrappers for the sm_90a features the convolution kernel uses:
+// cp.async, proxy fences and warpgroup MMA (wgmma) with shared-memory operand descriptors.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -11,108 +10,27 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// one lane of the (converged) warp: the tcgen05 / bulk-copy issue idiom
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-
-// ---------------------------------------------------------------- mbarrier
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void fence_mbar_init() {
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_n(uint32_t bar, uint32_t count) {        // `count` arrivals at once
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, 0x989680;\n\t"   // suspend-time hint: sleep in HW instead of spinning
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    while (!mbar_try_wait(bar, parity)) { }
-}
-
 // ---------------------------------------------------------------- async copies
-// 1-D bulk copy global -> shared, completion counted in bytes on an mbarrier (TMA engine, UBLKCP).
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
 // 16-byte cp.async with zero fill when src_bytes == 0 (LDGSTS).
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// generic-proxy smem writes -> visible to the async proxy (tcgen05.mma operand reads)
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
+    uint4 v;
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint4& v) {
+    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+
+// generic-proxy smem writes (st.shared, cp.async) -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 (fp16/bf16 operands, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// all previously issued MMAs of this thread -> arrive(1) on mbarrier when complete
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 256-bit global store (STG.E.ENL2.256, sm_100+): one full 32-byte sector per thread, so a strided NHWC epilogue does not
-// leave half-written sectors for L2 to complete with a DRAM read (profiles/r01m_conv_first*.ncu-rep: dram read = input + output)
-__device__ __forceinline__ void st_global_256(void* ptr, const uint4& a, const uint4& b) {
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(ptr), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b.x),
-                 "r"(b.y), "r"(b.z), "r"(b.w)
-                 : "memory");
 }
 
 // Read-only 128-bit global load under a predicate, zeros otherwise (no branch, no dependence on a dummy address).
@@ -125,81 +43,75 @@ __device__ __forceinline__ uint4 ldg128_if(const void* ptr, bool ok) {
     return v;
 }
 
-// ---------------------------------------------------------------- TMA tensor loads (UTMALDG)
-// 4-D tiled tensor load global -> shared (coordinates innermost first: channel, x, y, frame); out-of-bounds elements
-// (negative or past the tensor's extent, per dimension) are written as zeros; completion in bytes on an mbarrier.
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, int c0, int c1, int c2, int c3, uint32_t bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-        ::"r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
+// ---------------------------------------------------------------- wgmma
+// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle: rows of 128 B (64 fp16 of K), 8-row groups
+// `sbo_bytes` apart, the 16-byte chunk c of row r at r * 128 + ((c ^ (r & 7)) << 4) inside a 1024-byte aligned atom.
+// Adding 2 to the descriptor (32 bytes) steps to the next K16 slice of the row.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
+    d |= static_cast<uint64_t>(1) << 16;                 // leading byte offset: unused for swizzled K-major operands
+    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
+    d |= static_cast<uint64_t>(1) << 62;                 // SWIZZLE_128B
+    return d;
 }
 
-// ---------------------------------------------------------------- tcgen05 with the A operand in tensor memory
-// D[tmem] += A[tmem] * B[smem desc]; kind::f16.  A[m][k] lives in lane m, column k/2, half k%2 (tools/umma_ts_probe.cu).
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// registers -> TMEM: this warp's 32 lanes x N consecutive 32-bit columns (warp w may only touch lanes 32*(w%4)..+31)
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ void tmem_st2(uint32_t taddr, uint32_t a, uint32_t b) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1, %2};" ::"r"(taddr), "r"(a), "r"(b) : "memory");
-}
-__device__ __forceinline__ void tmem_st_zero32(uint32_t taddr) {
-    asm volatile(
-        "{\n\t.reg .b32 z;\n\tmov.b32 z, 0;\n\t"
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z, z};\n\t}"
-        ::"r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// ---------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle:
-// rows of 128 B (64 fp16), 8-row groups `sbo_bytes` apart.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t base_offset = 0) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= static_cast<uint64_t>(1) << 46;                 // descriptor version (Blackwell)
-    d |= static_cast<uint64_t>(base_offset & 7u) << 49;
-    d |= static_cast<uint64_t>(2) << 61;                 // SWIZZLE_128B
-    return d;
-}
-// (probe only, tools/umma_probe64.cu - a double-buffered 32-channel RIC variant built on it measured 15 % slower
-// than the 64-channel single-set producer and was dropped)  Same for 64-byte rows (32 fp16 of K), SWIZZLE_64B: 16-byte chunk index XOR ((row >> 1) & 3) on absolute
-// address bits [4:5] ^= [7:8]; 8-row groups are `sbo_bytes` apart (512 when rows are contiguous).
-__device__ __forceinline__ uint64_t umma_desc_sw64(uint32_t smem_addr, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(4) << 61;                 // SWIZZLE_64B
-    return d;
-}
-// K-major operand WITHOUT swizzle: 8-row x 16-byte core matrices.  Measured (tools/umma_probe_ns.cu): the MMA reads
-//     addr(row, k) = start + (row / 8) * sbo + (k / 8) * lbo + (row % 8) * 16 + (k % 8) * 2
-// for any 16-byte-aligned start and any 16-byte-multiple lbo / sbo, overlapping core matrices included - so
-// lbo = 16 over a pixel-linear buffer (16 B per pixel) makes "the next 8 K elements" simply "the next pixel".
-__device__ __forceinline__ uint64_t umma_desc_noswizzle(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    return d;
-}
-// Instruction descriptor: fp16 A/B (K-major), fp32 D, M x N tile.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t m, uint32_t n) {
-    return (1u << 4) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
+// D[64 x N] += A[64 x 16] * B[16 x N]; fp16 operands from shared memory (both K-major), fp32 accumulators in registers.
+// Thread t of the warpgroup holds d[i] = D[16 * (t / 32) + (t % 32) / 4 + 8 * ((i >> 1) & 1)][8 * (i >> 2) + 2 * (t % 4) + (i & 1)].
+template <int N>
+struct Wgmma;
+
+template <>
+struct Wgmma<32> {
+    __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(a), "l"(b));
+    }
+};
+
+template <>
+struct Wgmma<64> {
+    __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "l"(a), "l"(b));
+    }
+};
+
+template <>
+struct Wgmma<128> {
+    __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+            : "l"(a), "l"(b));
+    }
+};
 
 }  // namespace dsu

@@ -230,7 +230,7 @@ def stylize_character(root_dir: str, uid: str, pipeline=None, *, device="cuda:0"
 
 
 def main(argv=None) -> int:
-    ap = argparse.ArgumentParser(description="stage 1 + stage 2 over a character's blender_render tree on the B200 engine")
+    ap = argparse.ArgumentParser(description="stage 1 + stage 2 over a character's blender_render tree on the GPU engine")
     ap.add_argument("--root", default="../dataset/AnimatedDrawings/preprocessed", help="root_dir of the reference configs")
     ap.add_argument("--uid", required=True)
     ap.add_argument("--checkpoint_id", type=int, default=99999)

@@ -8,8 +8,8 @@ reference's ``test_stage1.py`` / ``test_stage2.py`` work unchanged once
 ``drawingspinup_b200.install()`` has rebound the two class names.
 
 The modules hold only parameters; ``forward`` hands raw device pointers to the hand-written
-sm_100a kernels through the C ABI (``include/dsu_b200.h``, ctypes).  No ``torch.nn.Conv2d``, no
-torch compute on the path, no CPU fallback: a missing library or a non-B200 device raises.
+sm_90a kernels through the C ABI (``include/dsu_b200.h``, ctypes).  No ``torch.nn.Conv2d``, no
+torch compute on the path, no CPU fallback: a missing library or a device other than sm_90 (H100) raises.
 """
 from __future__ import annotations
 
@@ -104,8 +104,8 @@ class _Generator(nn.Module):
         self.tanh = bool(tanh)
         self.filters = tuple(int(v) for v in filters)
         self.input_channels = int(input_channels)
-        # deterministic=True: bit-reproducible results run to run (stage 1 then issues its MMAs from ONE warp; by default six
-        # warps accumulate into one TMEM accumulator in a timing-dependent order, reproducible to ~1e-7 relative only)
+        # deterministic=True: bit-reproducible results run to run.  Every CTA accumulates its K chunks in a fixed order, so
+        # the engine is deterministic in both settings; the flag is kept for callers that request it explicitly.
         self.deterministic = bool(int(os.environ.get("DSU_DETERMINISTIC", "0"))) if deterministic is None else bool(deterministic)
         self.precision = precision or os.environ.get("DSU_PRECISION", "fp16x3")
         if self.precision not in capi.PRECISIONS:
@@ -179,7 +179,7 @@ class _Generator(nn.Module):
         """Create the engine for ``device`` if needed and (re)upload weights when any changed."""
         lib = capi.lib()
         if device.type != "cuda":
-            raise RuntimeError("drawingspinup_b200 generators run on a CUDA (B200) device only; got tensor on %s "
+            raise RuntimeError("drawingspinup_b200 generators run on a CUDA (H100, sm_90) device only; got tensor on %s "
                                "(no CPU fallback)" % device)
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if self._handle is None or self._handle_dev != idx:
@@ -199,8 +199,6 @@ class _Generator(nn.Module):
             h = C.c_void_p()
             capi.check(lib.dsu_create(C.byref(cfg), C.byref(h)), "dsu_create")
             self._handle, self._handle_dev = h, idx
-            if self.deterministic:
-                capi.check(lib.dsu_set_knob(h, b"tm_ni", 1), "dsu_set_knob(tm_ni)")
         sig = self._signature()
         if sig != self._loaded_sig:
             for key, t in self.state_dict().items():
@@ -327,15 +325,6 @@ class _Generator(nn.Module):
         if n < 0:
             capi.check(n, "dsu_profile_forward")
         return [(capi.lib().dsu_step_name(handle, i).decode(), ms[i], fl[i]) for i in range(min(n, cap))]
-
-    def watchdog_records(self):
-        """Test hook: decoded watchdog records of the tensor-memory RIC kernel (see dsu_debug_watchdog): list of
-        (warp, tag, a, b, block) for every warp that timed out in a barrier wait."""
-        if not self._handle:
-            return []
-        buf = (C.c_uint64 * 32)()
-        capi.lib().dsu_debug_watchdog(self._handle, buf, 32)
-        return [(i, (v >> 48) & 0xFF, (v >> 32) & 0xFFFF, (v >> 16) & 0xFFFF, v & 0xFFFF) for i, v in enumerate(buf) if v]
 
     def debug_buffer(self, buffer: int, plane: int, shape, dtype=torch.float16) -> torch.Tensor:
         """Test hook: host copy of an internal activation buffer (see dsu_debug_read)."""

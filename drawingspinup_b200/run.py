@@ -1,10 +1,10 @@
-"""Run an UNMODIFIED reference script on the B200 engine.
+"""Run an UNMODIFIED reference script on the CUDA engine.
 
     python -m drawingspinup_b200.run /path/to/3_style_translator/test_stage1.py --uid <uid>
 
 Changes into the script's folder (the scripts use relative ``configs/...`` paths,
 test_stage1.py:23), imports the reference's ``training.models``, rebinds ``GeneratorJ_RIC`` and
-``GeneratorJ`` to the B200 classes (see :func:`drawingspinup_b200.install`) and executes the script
+``GeneratorJ`` to the engine classes (see :func:`drawingspinup_b200.install`) and executes the script
 as ``__main__``.  Everything else in the script - YAML parsing, ``torch.load``,
 ``load_state_dict``, the DataLoader, PNG writing - is the reference's own code.
 """

@@ -1,4 +1,4 @@
-/* dsu_b200 - C ABI of the B200-native DrawingSpinUp stylization engine.
+/* dsu_b200 - C ABI of the DrawingSpinUp stylization engine (CUDA, sm_90a).
  *
  * The reference (LordLiang/DrawingSpinUp, 100 % Python) has no FFI: its seam for this path is
  * `training.trainers.build_model` -> `getattr(training.models, type)(**args)`
@@ -79,10 +79,9 @@ int dsu_loaded_keys(dsu_handle h);
  * tensor-core tiles, upload.  Requires every expected key (strict=True semantics). */
 int dsu_finalize(dsu_handle h, void* stream);
 
-/* Development / test hook, no counterpart in the reference: kernel-selection knobs of this handle ("first", "halo_ns",
- * "halo_ks", "tm_ni", "tm_sb", "derive_edge", "tm_trace", ... - engine.cu Knobs).  Their defaults are read once from the
- * environment (DSU_<NAME>) by dsu_create; "subpixel" and "n128" shape the launch plan / the weight packing and can only be set
- * through the environment (DSU_E_STATE otherwise). */
+/* Development / test hook, no counterpart in the reference: knobs of this handle ("first", "n128", "subpixel", "derive_edge" -
+ * engine.cu Knobs).  Their defaults are read once from the environment (DSU_<NAME>) by dsu_create; "subpixel" shapes the launch plan
+ * and can only be set through the environment (DSU_E_STATE otherwise). */
 int dsu_set_knob(dsu_handle h, const char* name, int32_t value);
 
 /* generate_coordinates (models.py:551-604) is data independent; by default the engine derives the
@@ -137,11 +136,6 @@ int dsu_compose_rgba(const float* y_dev, const float* mask_dev, int32_t B, int32
                      uint8_t* out_rgba_dev, void* stream);
 /* pos2edge (run_render.py:31-57): pos RGBA [B,H,W,4] -> edge [B,H,W] (255 on edges). */
 int dsu_pos2edge(const uint8_t* pos_dev, int32_t B, int32_t H, int32_t W, uint8_t* edge_dev, void* stream);
-
-/* Test hook: watchdog records of the tensor-memory RIC kernel (conv_ric_tm.cu).  A barrier wait that exceeds ~1 s (a
- * protocol bug) stores 0xD5<<56 | tag<<48 | a<<32 | b<<16 | block per warp in pinned host memory and traps; this copies the
- * first n slots (readable even after the launch failure) and returns how many are non-zero. */
-int dsu_debug_watchdog(dsu_handle h, uint64_t* out, int32_t n);
 
 /* Test hook: copy an internal activation buffer of the last forward to the host (synchronous).
  * buffer: 0 SK0(o0|x) 1 P0 2 O1 3 P1 4 O2 5 T 6 U 7 V2 8 V1 9 C11 10 S0 (fp16 NHWC), 100 = fp32 residual

@@ -16,7 +16,9 @@ What is recorded (all seeded, see drawingspinup_b200/synth.py):
   * ``DatasetFullImages.__getitem__`` (data.py:23-47) incl. the stage-2 edge burn-in, via real PNGs;
   * ``to_image_space`` (custom_transforms.py:7-8) known answers;
   * ``pos2edge`` (run_render.py:31-57; the function is extracted with ``ast`` because importing the
-    module needs Blender-side packages).
+    module needs Blender-side packages);
+  * the state-dict layout (keys in order, shapes, dtypes) of the modules ``training.trainers.build_model``
+    (trainers.py:33-35) returns for both generator classes (``GOLDEN_ONLY=build_model`` records only this).
 """
 from __future__ import annotations
 
@@ -52,7 +54,22 @@ def _no_cuda(fn, *a, **k):
         torch.Tensor.cuda = orig
 
 
+def build_model_layout():
+    """reference_state_dict_layout.npz: per class, the keys, shapes (padded with -1) and dtypes of build_model(...).state_dict()."""
+    import training.trainers as rt
+    out = {}
+    for name in ("GeneratorJ", "GeneratorJ_RIC"):
+        sd = rt.build_model(name, dict(ARGS), "cpu").state_dict()
+        out["keys_" + name] = np.array(list(sd.keys()))
+        out["shapes_" + name] = np.array([list(v.shape) + [-1] * (4 - v.dim()) for v in sd.values()], dtype=np.int64)
+        out["dtypes_" + name] = np.array([str(v.dtype) for v in sd.values()])
+    np.savez_compressed(os.path.join(OUT, "reference_state_dict_layout.npz"), **out)
+
+
 def main():
+    if os.environ.get("GOLDEN_ONLY", "") == "build_model":
+        build_model_layout()
+        return
     import training.models as rm
     from training.data import DatasetFullImages
     from training.custom_transforms import to_image_space
@@ -147,6 +164,7 @@ def main():
             cv2.imwrite(path, p64[i][..., [2, 1, 0, 3]])       # RGBA array -> BGRA file order
             edges.append(ns["pos2edge"](path))
     np.savez_compressed(os.path.join(OUT, "pos2edge.npz"), pos=p64, edges=np.stack(edges))
+    build_model_layout()
     print("golden fixtures written to", OUT)
 
 

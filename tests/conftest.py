@@ -15,7 +15,7 @@ VARIANT_ARGS = dict(use_bias=True, tanh=False, append_smoothers=False, resnet_bl
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (B200) device; run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (H100, sm_90) device; run with -m gpu on a GPU machine")
 
 
 @pytest.fixture(scope="session")
