@@ -55,6 +55,7 @@ SYMBOLS = {
     "dsu_pos2edge": (C.c_int, [_VP, _I32, _I32, _I32, _VP, _VP]),
     "dsu_profile_forward": (C.c_int, [_VP, _I32, _I32, _I32, _I32, _VP, C.POINTER(C.c_double), C.POINTER(C.c_double), _I32]),
     "dsu_step_name": (C.c_char_p, [_VP, _I32]),
+    "dsu_step_kernel": (C.c_char_p, [_VP, _I32]),
     "dsu_debug_read": (C.c_int, [_VP, _I32, _I32, _VP, _SZ]),
 }
 

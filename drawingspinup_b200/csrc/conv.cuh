@@ -18,13 +18,15 @@ constexpr int kMaxSeg = 6;      // concat segments (second half = lo planes in e
 
 // One 16-byte (8-channel) K slot: which tap of which source segment fills it.
 // plain conv: one entry per (chunk, slot).  RIC conv: one entry per (64-channel block, slot) - the
-// tap is the chunk's position inside the block.
+// tap is the chunk's position inside the block.  Halo mode: per chunk as for a plain conv, plus one entry per
+// (channel block, 16-byte slot of a halo pixel) saying what the halo holds (ConvParams::hslots).
 struct Slot {
     int8_t dy, dx;      // plain: tap offset (kh - pad, kw - pad)
     uint8_t seg;        // source segment index (lo plane = seg + kMaxSeg/2)
     uint8_t valid;      // 0 -> zero fill (K padding)
     uint16_t choff;     // first channel inside the segment buffer
-    uint16_t pad_;
+    uint8_t hslot;      // halo mode: the 16-byte slot of the halo pixel that holds these 8 channels
+    uint8_t pad_;
 };
 static_assert(sizeof(Slot) == 8, "Slot must be 8 bytes");
 
@@ -93,9 +95,11 @@ struct ConvParams {
     // source whose output pixel (oy, ox) of the Hout x Wout grid lands at (2*oy + sub_py, 2*ox + sub_px) of the
     // (2*Hout) x (2*Wout) output buffer
     int sub, sub_py, sub_px;
-    // first layer (one 8-channel segment, stride 1): stage the (kTileH + ksize - 1) x (kTileW + ksize - 1) input halo of the
-    // tile once in shared memory and build every A chunk from it instead of from global memory
-    int halo, ksize, pad;
+    // halo mode (stride 1, no fused upsampling, not RIC): the channels are walked in blocks of 128 bytes per pixel; the
+    // (tile rows + ksize - 1) x (kTileW + ksize - 1) input halo of each block, origin (ty0 - pad_y, tx0 - pad_x), is staged in
+    // shared memory once and the A fragments of every tap are read from it straight into registers
+    int halo, ksize, pad_y, pad_x;
+    const Slot* hslots;     // [nblocks][8]: the channels of each 16-byte slot of a halo pixel
     int n128;               // Cout a multiple of 128: issue N = 128 wgmma instructions (else N = 64 / 32)
 };
 

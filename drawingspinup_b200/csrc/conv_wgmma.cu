@@ -1,20 +1,28 @@
 // Fused convolution as an implicit GEMM on the Hopper tensor cores (wgmma, fp32 accumulators in registers).
 //
-// One CTA computes a kTileH x kTileW patch (128 output pixels = GEMM M) of one frame for all Cout channels (GEMM N).
-// K = taps x input channels, walked in 64-element chunks through a kStages-deep ring of shared-memory stages; each
-// stage holds the A operand (one 128-byte SWIZZLE_128B row per output pixel) and the chunk's pre-swizzled weight tile
-// (B operand, one 128-byte row per output channel).  Both warpgroups (256 threads) do everything in turn:
-//   * PRODUCE chunk q + 2 while the MMAs of chunk q run.  Each 16-byte slot of an A row is 8 channels of one tap of one
-//     concat segment (slot table), so plain 3x3 / 7x7 taps, stride 2, fused nearest-x2 upsampling, sub-pixel classes
-//     and channel concatenation are pure address arithmetic (cp.async with zero fill at the border).  The first layer
-//     (one 8-channel segment, stride 1) stages the tile's input halo in shared memory once and builds its A chunks from
-//     there (49 taps of the 7x7 conv0 read each input pixel 49 times).  RIC (stage-1
-//     deformable) layers blend the four bilinear corners of the rotated tap in registers and store the result.
-//     The weight tile is streamed with cp.async.
+// One CTA computes a tile of output pixels (GEMM M) of one frame for all Cout channels (GEMM N), K = taps x input
+// channels walked in 64-element chunks.  Two warpgroups (256 threads) do everything in turn.  Two mainloops:
+//
+// conv_wgmma_kernel (tap / RIC modes): a kTileH x kTileW patch (128 pixels).  Each chunk goes through a kStages-deep
+// ring of shared-memory stages holding the A operand (one 128-byte SWIZZLE_128B row per output pixel) and the chunk's
+// pre-swizzled weight tile (B operand, one 128-byte row per output channel).
+//   * PRODUCE chunk q + 2 while the MMAs of chunk q run.  Tap mode: each 16-byte slot of an A row is 8 channels of one
+//     tap of one concat segment (slot table), so stride 2 and fused nearest-x2 upsampling are pure address arithmetic
+//     (cp.async with zero fill at the border).  RIC (stage-1 deformable) layers blend the four bilinear corners of the
+//     rotated tap in registers and store the result.  The weight tile is streamed with cp.async.
 //   * ISSUE wgmma: warpgroup w multiplies A rows 64w .. 64w+63 by the whole weight tile into its register accumulators.
-//   * after the last chunk, STAGE the accumulators to shared memory as fp32 rows and run the fused epilogue: folded BN /
-//     activation / residual, fp16 NHWC (hi [+lo] planes), fp32 activations, the fp32 residual stream, or the conv_12
-//     1x1 + tanh + uint8 composite tail (one pixel row per thread, two threads per row).
+//
+// conv_halo_kernel (halo mode): the planner (engine.cu compile_layer) sends the first layer and every other stride-1 layer
+// without fused upsampling whose Cout <= 64 here, sub-pixel classes included.  A kRows x kTileW patch: kRows = 16 for
+// Cout <= 64; the first layer wider than 64 channels runs on 8-row tiles (register budget).  The concat is walked in channel blocks of
+// 128 bytes per pixel (8 groups of 8 channels, or 4 groups as hi + lo in exact mode).  The tile's input halo of a block
+// is loaded once with cp.async (double-buffered: block b + 1 lands while the taps of block b run) and every chunk's A
+// fragments are read from it with ldmatrix straight into registers (wgmma RS form, double-buffered across chunks), so
+// an input pixel crosses L2 once per block instead of once per tap.  Weight tiles stream through the same ring as above.
+//
+// After the last chunk both kernels STAGE the accumulators to shared memory as fp32 rows and run the fused epilogue:
+// folded BN / activation / residual, fp16 NHWC (hi [+lo] planes), fp32 activations, the fp32 residual stream, or the
+// conv_12 1x1 + tanh + uint8 composite tail (one pixel row per thread, two threads per row).
 // "Exact" mode (split fp16): a K chunk holds 32 channels as [a_hi | a_lo], its weight tile [W_hi | W_lo] in one
 // 128-byte row; A steps 0-3 are issued against B steps 0,1,0,1 and A steps 0,1 again against B steps 2,3 into the
 // same accumulator: a_hi*W_hi + a_lo*W_hi + a_hi*W_lo, fp32-grade products at 3x the tensor work.
@@ -24,64 +32,50 @@ namespace dsu {
 
 namespace {
 
-constexpr int kModeTap = 0, kModeRic = 1, kModeRicExact = 2, kModeHalo = 3;
+constexpr int kModeTap = 0, kModeRic = 1, kModeRicExact = 2;
 
 struct SmemLayout {
     uint32_t stage_bytes;   // A tile + B tile
     uint32_t par;           // epilogue parameters, after the ring (the staged accumulators reuse the ring)
-    uint32_t halo;          // first-layer input halo (hi plane, then the lo plane in exact mode)
     uint32_t total;         // from the 1024-aligned base
 };
 
-// pixels of the first-layer halo of one tile
-__host__ __device__ inline int halo_pixels(int ksize) { return (kTileH + ksize - 1) * (kTileW + ksize - 1); }
-
 __host__ __device__ inline uint32_t acc_pitch(int cout) { return static_cast<uint32_t>(cout) + 4; }   // floats per staged row
 
-__host__ __device__ inline SmemLayout smem_layout(int cout, int b_bytes, uint32_t halo_bytes) {
+__host__ __device__ inline uint32_t par_bytes(int cout) { return (7 * cout + 4) * 4; }
+
+__host__ __device__ inline SmemLayout smem_layout(int cout, int b_bytes) {
     SmemLayout L;
     L.stage_bytes = kABytes + b_bytes;
     const uint32_t ring = kStages * L.stage_bytes, staged = kTileM * acc_pitch(cout) * 4;
     L.par = ((ring > staged ? ring : staged) + 15u) & ~15u;
-    L.halo = (L.par + (7 * cout + 4) * 4 + 15u) & ~15u;
-    L.total = L.halo + halo_bytes;
+    L.total = L.par + par_bytes(cout);
     return L;
 }
 
-__host__ __device__ inline uint32_t halo_bytes(const ConvParams& p) {
-    return p.halo ? static_cast<uint32_t>(halo_pixels(p.ksize)) * 16u * (p.exact ? 2u : 1u) : 0u;
-}
+// halo mode: output rows per tile.  16 x 16 tiles halve the weight traffic per pixel; above 64 channels the two m64 blocks
+// per warpgroup would not fit the register file next to the accumulators, so those layers keep 8 x 16.
+__host__ __device__ inline int halo_rows(int cout) { return cout <= 64 ? 16 : 8; }
 
-// ---- first layer: the tile's (kTileH + k - 1) x (kTileW + k - 1) input pixels (8 channels, hi [+ lo] plane) with cp.async,
-// zeros outside the image.  Every slot of the single segment reads the same 8 channels (choff of slot 0).
-__device__ __forceinline__ void load_halo(const ConvParams& p, uint32_t halo, int tid, int n, int ty0, int tx0) {
-    const int hw = kTileW + p.ksize - 1, npix = halo_pixels(p.ksize);
-    const size_t frame_in = static_cast<size_t>(n) * p.Hin * p.Win;
-    const int choff = p.slots[0].choff;
-    for (int i = tid; i < npix * (p.exact ? 2 : 1); i += kThreads) {
-        const int plane = i >= npix, pix = i - plane * npix;
-        const int y = ty0 - p.pad + pix / hw, x = tx0 - p.pad + pix % hw;
-        const bool ok = static_cast<unsigned>(y) < static_cast<unsigned>(p.Hin) && static_cast<unsigned>(x) < static_cast<unsigned>(p.Win);
-        const Seg sg = p.seg[plane ? kMaxSeg / 2 : 0];
-        const __half* src = sg.ptr + choff + (ok ? (frame_in + static_cast<size_t>(y) * p.Win + x) * sg.pitch : 0);
-        cp_async16(halo + 16u * i, src, ok ? 16u : 0u);
-    }
-}
+struct HaloLayout {
+    uint32_t stage_bytes;   // B tile of one chunk (ring of kStages at offset 0)
+    uint32_t halo;          // two halo buffers of halo_bytes
+    uint32_t halo_bytes;    // (rows + k - 1) x (kTileW + k - 1) pixels x 128 B
+    uint32_t zero;          // 16 zero bytes: the A rows of K-padding slots
+    uint32_t par;           // epilogue parameters (the staged accumulators reuse ring + halos)
+    uint32_t total;
+};
 
-// ---- first layer: chunk q's A rows copied out of the halo (same slot table and row mapping as tap mode)
-__device__ __forceinline__ void produce_halo(const ConvParams& p, int q, uint32_t a, uint32_t halo, int tid) {
-    const int j = tid & 7, prow = tid >> 3;
-    const Slot sl = p.slots[q * 8 + j];
-    const int hw = kTileW + p.ksize - 1;
-    const uint32_t plane = sl.seg >= kMaxSeg / 2 ? static_cast<uint32_t>(halo_pixels(p.ksize)) * 16u : 0u;
-    const uint32_t dst0 = a + static_cast<uint32_t>(prow) * 128u + (static_cast<uint32_t>(j ^ (prow & 7)) << 4);
-    const int hx = (prow & 15) + sl.dx + p.pad;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int hy = (prow >> 4) + 2 * i + sl.dy + p.pad;
-        const uint4 v = sl.valid ? ld_shared_v4(halo + plane + 16u * static_cast<uint32_t>(hy * hw + hx)) : make_uint4(0u, 0u, 0u, 0u);
-        st_shared_v4(dst0 + i * 4096u, v);
-    }
+__host__ __device__ inline HaloLayout halo_layout(int cout, int rows, int ksize) {
+    HaloLayout L;
+    L.stage_bytes = static_cast<uint32_t>(cout) * 128u;
+    L.halo = kStages * L.stage_bytes;
+    L.halo_bytes = static_cast<uint32_t>((rows + ksize - 1) * (kTileW + ksize - 1)) * 128u;
+    L.zero = L.halo + 2 * L.halo_bytes;
+    const uint32_t main_end = L.zero + 16u, staged = static_cast<uint32_t>(rows * kTileW) * acc_pitch(cout) * 4u;
+    L.par = ((main_end > staged ? main_end : staged) + 15u) & ~15u;
+    L.total = L.par + par_bytes(cout);
+    return L;
 }
 
 __device__ __forceinline__ constexpr int ric_r0(int m) { return (m >= 2 && m <= 5) ? 0 : 1; }   // first corner row - 1 + 1
@@ -197,14 +191,17 @@ __device__ __forceinline__ void produce_ric(const ConvParams& p, int q, uint32_t
     }
 }
 
-template <int kMode>
-__device__ __forceinline__ void produce(const ConvParams& p, int q, uint32_t stage, uint32_t halo, int tid, int n, int ty0, int tx0) {
-    if constexpr (kMode == kModeTap) produce_tap(p, q, stage, tid, n, ty0, tx0);
-    else if constexpr (kMode == kModeHalo) produce_halo(p, q, stage, halo, tid);
-    else produce_ric<kMode == kModeRicExact>(p, q, stage, tid, n, ty0, tx0);
-    // weight tile of chunk q
+// weight tile of chunk q (cp.async)
+__device__ __forceinline__ void produce_b(const ConvParams& p, int q, uint32_t dst, int tid) {
     const uint8_t* src = p.wpack + static_cast<size_t>(q) * p.b_bytes;
-    for (int i = tid; i < p.b_bytes / 16; i += kThreads) cp_async16(stage + kABytes + 16u * i, src + 16 * i, 16u);
+    for (int i = tid; i < p.b_bytes / 16; i += kThreads) cp_async16(dst + 16u * i, src + 16 * i, 16u);
+}
+
+template <int kMode>
+__device__ __forceinline__ void produce(const ConvParams& p, int q, uint32_t stage, int tid, int n, int ty0, int tx0) {
+    if constexpr (kMode == kModeTap) produce_tap(p, q, stage, tid, n, ty0, tx0);
+    else produce_ric<kMode == kModeRicExact>(p, q, stage, tid, n, ty0, tx0);
+    produce_b(p, q, stage + kABytes, tid);
 }
 
 // the K steps of one chunk: every PN-column piece of the accumulator against the matching PN rows of the weight tile
@@ -230,6 +227,96 @@ __device__ __forceinline__ void mma_chunk(float* acc, uint64_t da, uint64_t db, 
     }
 }
 
+// the same K steps with A from registers: a[mb][k] = K step k of m64 block mb; in split-fp16 the hi fragments (steps 0-1)
+// are used for both a_hi*W_hi and a_hi*W_lo.  Every step is issued, also in the ragged last chunk: its K-padding slots
+// read zeros against zero weights and add exact zeros, and a branch-free sequence keeps the wgmmas back to back.
+template <int NC, int PN, int MB, bool kExact>
+__device__ __forceinline__ void mma_chunk_rs(float (*acc)[NC / 2], const uint32_t (*a)[4][4], uint64_t db) {
+    constexpr uint64_t kPieceStep = PN * 128 / 16;
+    auto step = [&](int ka, int kb) {
+#pragma unroll
+        for (int mb = 0; mb < MB; ++mb)
+#pragma unroll
+            for (int j = 0; j < NC / PN; ++j) Wgmma<PN>::mma_rs(acc[mb] + j * (PN / 2), a[mb][ka], db + 2 * kb + j * kPieceStep);
+    };
+#pragma unroll
+    for (int k = 0; k < 4; ++k) step(k, kExact ? (k & 1) : k);
+    if constexpr (kExact) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k) step(k, 2 + k);
+    }
+}
+
+// ---- halo mode: the input halo of channel block `blk` with cp.async, zeros outside the image.  Pixel-major, 128 B per
+// pixel, 16-byte slot s at ((s ^ (pixel & 7)) << 4): any 8 consecutive halo pixels are bank-conflict free for ldmatrix.
+template <int kRows>
+__device__ __forceinline__ void load_halo(const ConvParams& p, int blk, uint32_t halo, int tid, int n, int ty0, int tx0) {
+    const int hw = kTileW + p.ksize - 1, npix = (kRows + p.ksize - 1) * hw;
+    const int s = tid & 7;                                // the 8 threads of a pixel copy its 128 contiguous bytes
+    const Slot sl = p.hslots[blk * 8 + s];
+    const Seg sg = p.seg[sl.seg];
+    const __half* sbase = sg.ptr + sl.choff;
+    const size_t frame_in = static_cast<size_t>(n) * p.Hin * p.Win;
+    for (int pix = tid >> 3; pix < npix; pix += kThreads / 8) {
+        const int hy = pix / hw, hx = pix - hy * hw;
+        const int y = ty0 - p.pad_y + hy, x = tx0 - p.pad_x + hx;
+        const bool ok = sl.valid && static_cast<unsigned>(y) < static_cast<unsigned>(p.Hin) && static_cast<unsigned>(x) < static_cast<unsigned>(p.Win);
+        const __half* src = ok ? sbase + (frame_in + static_cast<size_t>(y) * p.Win + x) * sg.pitch : sbase;
+        cp_async16(halo + static_cast<uint32_t>(pix) * 128u + (static_cast<uint32_t>(s ^ (pix & 7)) << 4), src, ok ? 16u : 0u);
+    }
+}
+
+// ---- halo mode: chunk q's A fragments of this warp (rows pb[mb] of each m64 block) from the halo into registers.  Lanes
+// 0-15 address the 16 rows of slot 2k, lanes 16-31 those of slot 2k + 1; each slot reads its halo pixel shifted by its own
+// tap, so taps of several channel groups may share a chunk.  K-padding slots read 16 zero bytes.
+template <int MB>
+__device__ __forceinline__ void load_a(const ConvParams& p, int q, uint32_t halo, uint32_t zero, const int* pb, int lane,
+                                       uint32_t (*a)[4][4]) {
+    const int hw = kTileW + p.ksize - 1;
+    const uint2* slots = reinterpret_cast<const uint2*>(p.slots) + q * 8 + (lane >> 4);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint2 raw = __ldg(slots + 2 * k);
+        Slot sl;
+        memcpy(&sl, &raw, sizeof(sl));
+        const int shift = (sl.dy + p.pad_y) * hw + sl.dx + p.pad_x;
+#pragma unroll
+        for (int mb = 0; mb < MB; ++mb) {
+            const int pix = pb[mb] + shift;
+            const uint32_t addr = sl.valid ? halo + static_cast<uint32_t>(pix) * 128u + (static_cast<uint32_t>(sl.hslot ^ (pix & 7)) << 4) : zero;
+            ldsm_x4(a[mb][k], addr);
+        }
+    }
+}
+
+// accumulators (MB m64 blocks per warpgroup) -> fp32 rows in shared memory -> fused epilogue, one pixel row per thread pair
+template <int NC, int MB>
+__device__ __forceinline__ void store_tile(const ConvParams& p, uint8_t* smem, const float* s_par, float (*acc)[NC / 2],
+                                           int tid, int n, int ty0, int tx0) {
+    constexpr int kM = 128 * MB;
+    float* staged = reinterpret_cast<float*>(smem);
+    {
+        const int wg = tid >> 7, w = (tid >> 5) & 3, l = tid & 31;
+#pragma unroll
+        for (int mb = 0; mb < MB; ++mb) {
+            const int r0 = wg * (kM / 2) + mb * 64 + 16 * w + (l >> 2), c0 = 2 * (l & 3);
+#pragma unroll
+            for (int i = 0; i < NC / 2; i += 2) {
+                const int r = r0 + 8 * ((i >> 1) & 1), c = c0 + 8 * (i >> 2);
+                *reinterpret_cast<float2*>(staged + r * acc_pitch(NC) + c) = make_float2(acc[mb][i], acc[mb][i + 1]);
+            }
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < MB; ++i) {
+        const int r = (tid & 127) + 128 * i;              // patch pixel; two threads per row split the 32-column batches
+        const float* row = staged + r * acc_pitch(NC);
+        if (p.sub) epilogue_row<kEpiAll, true>(p, s_par, row, n, ty0 + (r >> 4), tx0 + (r & 15), tid >> 7);
+        else epilogue_row<kEpiAll, false>(p, s_par, row, n, ty0 + (r >> 4), tx0 + (r & 15), tid >> 7);
+    }
+}
+
 }  // namespace
 
 // NC = Cout, PN = wgmma N per instruction (a divisor of NC: 32, 64 or 128)
@@ -240,8 +327,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     const uint32_t raw_u32 = smem_u32(smem_raw);
     const uint32_t base = (raw_u32 + 1023u) & ~1023u;     // SWIZZLE_128B atoms are 1024-byte aligned
     uint8_t* smem = smem_raw + (base - raw_u32);
-    const SmemLayout L = smem_layout(NC, p.b_bytes, halo_bytes(p));
-    const uint32_t halo = base + L.halo;
+    const SmemLayout L = smem_layout(NC, p.b_bytes);
     float* s_par = reinterpret_cast<float*>(smem + L.par);
 
     const int tid = threadIdx.x;
@@ -250,25 +336,19 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     const int ty0 = blockIdx.y * kTileH;
     const int tx0 = blockIdx.x * kTileW;
     const int nq = p.nchunks;
-    // chunks with the ragged K tail: the last one (tap / halo mode) or the 9 taps of the last channel block (RIC)
+    // chunks with the ragged K tail: the last one (tap mode) or the 9 taps of the last channel block (RIC)
     const int tail_from = (kMode == kModeRic || kMode == kModeRicExact) ? (p.nblocks - 1) * 9 : nq - 1;
 
     load_epilogue_params(p, s_par, tid, kThreads);
 
-    float acc[NC / 2];
+    float acc[1][NC / 2];
 #pragma unroll
-    for (int i = 0; i < NC / 2; ++i) acc[i] = 0.0f;
+    for (int i = 0; i < NC / 2; ++i) acc[0][i] = 0.0f;
 
-    if constexpr (kMode == kModeHalo) {                   // the halo must be complete before any chunk is built from it
-        load_halo(p, halo, tid, n, ty0, tx0);
-        cp_async_commit();
-        cp_async_wait<0>();
-        __syncthreads();
-    }
     // prologue: chunks 0 and 1; every iteration commits one cp.async group so that "chunk q has landed" is wait_group 1
 #pragma unroll
     for (int s = 0; s < kStages - 2; ++s) {
-        if (s < nq) produce<kMode>(p, s, base + s * L.stage_bytes, halo, tid, n, ty0, tx0);
+        if (s < nq) produce<kMode>(p, s, base + s * L.stage_bytes, tid, n, ty0, tx0);
         cp_async_commit();
     }
     for (int q = 0; q < nq; ++q) {
@@ -279,74 +359,161 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
         const uint64_t da = wgmma_desc_sw128(stage + wg * (kABytes / 2), 1024), db = wgmma_desc_sw128(stage + kABytes, 1024);
         const bool tail = q >= tail_from;
         wgmma_fence();
-        mma_chunk<NC, PN>(acc, da, db, tail ? p.kmask_last : p.kmask_full, tail ? p.kmask2_last : p.kmask2_full);
+        mma_chunk<NC, PN>(acc[0], da, db, tail ? p.kmask_last : p.kmask_full, tail ? p.kmask2_last : p.kmask2_full);
         wgmma_commit();
         wgmma_wait<1>();                                  // this warpgroup's MMAs of chunk q - 1 have retired
-        if (q + kStages - 2 < nq) produce<kMode>(p, q + kStages - 2, base + ((q + kStages - 2) % kStages) * L.stage_bytes, halo, tid, n, ty0, tx0);
+        if (q + kStages - 2 < nq) produce<kMode>(p, q + kStages - 2, base + ((q + kStages - 2) % kStages) * L.stage_bytes, tid, n, ty0, tx0);
         cp_async_commit();
     }
     wgmma_wait<0>();
     cp_async_wait<0>();
     __syncthreads();                                      // the ring is free: stage the accumulators over it
+    store_tile<NC, 1>(p, smem, s_par, acc, tid, n, ty0, tx0);
+}
 
-    {
-        float* staged = reinterpret_cast<float*>(smem);
-        const int w = (tid >> 5) & 3, l = tid & 31;
-        const int r0 = wg * 64 + 16 * w + (l >> 2), c0 = 2 * (l & 3);
+// Halo mode.  Chunk q belongs to channel block q / k^2 (every block but the last has exactly k^2 chunks, one per tap; the
+// last one may pack several taps of its few channel groups into a chunk).  Per iteration q: wait for the weight tile of
+// chunk q, issue its MMAs with the A fragments already in registers, wait for the MMAs of chunk q - 1 (their registers
+// are free), ldmatrix the fragments of chunk q + 1, start the weight tile of chunk q + 2 and, in the first iteration of
+// block b, the halo of block b + 1 (it lands k^2 - 2 iterations before it is read; the buffer it overwrites was last
+// read in iteration b k^2 - 2).  The chunk loop is unrolled by two so that the fragment buffers have fixed registers.
+template <int NC, int PN, int kRows, bool kExact>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_halo_kernel(const __grid_constant__ ConvParams p) {
+    constexpr int kM = kRows * kTileW, MB = kM / 128;     // m64 blocks per warpgroup
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t raw_u32 = smem_u32(smem_raw);
+    const uint32_t base = (raw_u32 + 1023u) & ~1023u;
+    uint8_t* smem = smem_raw + (base - raw_u32);
+    const HaloLayout L = halo_layout(NC, kRows, p.ksize);
+    float* s_par = reinterpret_cast<float*>(smem + L.par);
+    const uint32_t zero = base + L.zero;
+
+    const int tid = threadIdx.x;
+    const int wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+    const int n = blockIdx.z;
+    const int ty0 = blockIdx.y * kRows;
+    const int tx0 = blockIdx.x * kTileW;
+    const int nq = p.nchunks, kk = p.ksize * p.ksize;
+    const int hw = kTileW + p.ksize - 1;
+
+    load_epilogue_params(p, s_par, tid, kThreads);
+    if (tid < 4) reinterpret_cast<uint32_t*>(smem + L.zero)[tid] = 0u;
+
+    // halo pixel of this lane's A row in each m64 block, for the tap (0, 0) of the halo origin
+    int pb[MB];
 #pragma unroll
-        for (int i = 0; i < NC / 2; i += 2) {
-            const int r = r0 + 8 * ((i >> 1) & 1), c = c0 + 8 * (i >> 2);
-            *reinterpret_cast<float2*>(staged + r * acc_pitch(NC) + c) = make_float2(acc[i], acc[i + 1]);
-        }
+    for (int mb = 0; mb < MB; ++mb) {
+        const int r = wg * (kM / 2) + mb * 64 + warp * 16 + (lane & 15);
+        pb[mb] = (r >> 4) * hw + (r & 15);
     }
-    __syncthreads();
-    {
-        const int r = tid & (kTileM - 1);                 // patch pixel; two threads per row split the 32-column batches
-        const float* row = reinterpret_cast<const float*>(smem) + r * acc_pitch(NC);
-        if (p.sub) epilogue_row<kEpiAll, true>(p, s_par, row, n, ty0 + (r >> 4), tx0 + (r & 15), tid >> 7);
-        else epilogue_row<kEpiAll, false>(p, s_par, row, n, ty0 + (r >> 4), tx0 + (r & 15), tid >> 7);
+    float acc[MB][NC / 2];
+#pragma unroll
+    for (int mb = 0; mb < MB; ++mb)
+#pragma unroll
+        for (int i = 0; i < NC / 2; ++i) acc[mb][i] = 0.0f;
+    uint32_t a[2][MB][4][4];                              // [buffer][m64 block][K step][register]
+
+    auto halo_buf = [&](int blk) { return base + L.halo + static_cast<uint32_t>(blk & 1) * L.halo_bytes; };
+    // prologue: halo of block 0 + weights of chunk 0, then weights of chunk 1 (one cp.async group each)
+    load_halo<kRows>(p, 0, halo_buf(0), tid, n, ty0, tx0);
+    produce_b(p, 0, base, tid);
+    cp_async_commit();
+    if (nq > 1) produce_b(p, 1, base + L.stage_bytes, tid);
+    cp_async_commit();
+    cp_async_wait<1>();
+    __syncthreads();                                      // halo 0 (and the zero row) visible to every warp
+    load_a<MB>(p, 0, halo_buf(0), zero, pb, lane, a[0]);
+
+    auto step = [&](int q, const uint32_t (*cur)[4][4], uint32_t (*nxt)[4][4]) {
+        cp_async_wait<kStages - 3>();
+        fence_proxy_async_smem();
+        __syncthreads();                                  // weights of chunk q landed; the MMAs of chunk q - 2 have retired
+        const uint64_t db = wgmma_desc_sw128(base + (q % kStages) * L.stage_bytes, 1024);
+        wgmma_fence();
+        mma_chunk_rs<NC, PN, MB, kExact>(acc, cur, db);
+        wgmma_commit();
+        wgmma_wait<1>();                                  // the MMAs of chunk q - 1 have retired: `nxt` is free
+        if (q + 1 < nq) load_a<MB>(p, q + 1, halo_buf((q + 1) / kk), zero, pb, lane, nxt);
+        if (q + 2 < nq) produce_b(p, q + 2, base + ((q + 2) % kStages) * L.stage_bytes, tid);
+        const int blk = q / kk;
+        if (q == blk * kk && blk + 1 < p.nblocks) load_halo<kRows>(p, blk + 1, halo_buf(blk + 1), tid, n, ty0, tx0);
+        cp_async_commit();
+    };
+    for (int q = 0; q < nq; q += 2) {
+        step(q, a[0], a[1]);
+        if (q + 1 < nq) step(q + 1, a[1], a[0]);
     }
+    wgmma_wait<0>();
+    cp_async_wait<0>();
+    __syncthreads();                                      // ring and halos are free: stage the accumulators over them
+    store_tile<NC, MB>(p, smem, s_par, acc, tid, n, ty0, tx0);
 }
 
 size_t conv_smem_bytes(const ConvParams& p) {
-    return smem_layout(p.Cout, p.b_bytes, halo_bytes(p)).total + 1024;
+    const uint32_t total = p.halo ? halo_layout(p.Cout, halo_rows(p.Cout), p.ksize).total : smem_layout(p.Cout, p.b_bytes).total;
+    return total + 1024;
 }
 
 namespace {
 
-template <int NC, int PN, int kMode>
-cudaError_t launch_nc(const ConvParams& p, cudaStream_t stream) {
-    // one flag per device: the attribute is per function and context
-    static bool attr_set[64] = {};
+// the attribute is per function and context: one flag per device
+template <typename K>
+cudaError_t allow_smem(K kernel, bool* attr_set) {
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
-    const size_t smem = conv_smem_bytes(p);
-    if (dev >= 64 || !attr_set[dev]) {
-        e = cudaFuncSetAttribute(conv_wgmma_kernel<NC, PN, kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return e;
-        if (dev < 64) attr_set[dev] = true;
-    }
+    if (dev < 64 && attr_set[dev]) return cudaSuccess;
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e == cudaSuccess && dev < 64) attr_set[dev] = true;
+    return e;
+}
+
+template <int NC, int PN, int kMode>
+cudaError_t launch_nc(const ConvParams& p, cudaStream_t stream) {
+    static bool attr_set[64] = {};
+    cudaError_t e = allow_smem(conv_wgmma_kernel<NC, PN, kMode>, attr_set);
+    if (e != cudaSuccess) return e;
     dim3 grid((p.Wout + kTileW - 1) / kTileW, (p.Hout + kTileH - 1) / kTileH, p.B);
-    conv_wgmma_kernel<NC, PN, kMode><<<grid, kThreads, smem, stream>>>(p);
+    conv_wgmma_kernel<NC, PN, kMode><<<grid, kThreads, conv_smem_bytes(p), stream>>>(p);
     return cudaGetLastError();
+}
+
+template <int NC, int PN, bool kExact>
+cudaError_t launch_halo_nc(const ConvParams& p, cudaStream_t stream) {
+    constexpr int kRows = NC <= 64 ? 16 : 8;              // halo_rows(NC)
+    static bool attr_set[64] = {};
+    cudaError_t e = allow_smem(conv_halo_kernel<NC, PN, kRows, kExact>, attr_set);
+    if (e != cudaSuccess) return e;
+    dim3 grid((p.Wout + kTileW - 1) / kTileW, (p.Hout + kRows - 1) / kRows, p.B);
+    conv_halo_kernel<NC, PN, kRows, kExact><<<grid, kThreads, conv_smem_bytes(p), stream>>>(p);
+    return cudaGetLastError();
+}
+
+// halo mode in fp16 / split fp16 (same numbering as the tap / RIC modes of launch_nc)
+constexpr int kModeHaloFp16 = 3, kModeHaloExact = 4;
+
+template <int kMode, int NC, int PN>
+cudaError_t launch_one(const ConvParams& p, cudaStream_t stream) {
+    if constexpr (kMode == kModeHaloFp16 || kMode == kModeHaloExact) return launch_halo_nc<NC, PN, kMode == kModeHaloExact>(p, stream);
+    else return launch_nc<NC, PN, kMode>(p, stream);
 }
 
 template <int kMode>
 cudaError_t launch_mode(const ConvParams& p, cudaStream_t stream) {
     switch (p.Cout) {
-        case 32: return launch_nc<32, 32, kMode>(p, stream);
-        case 64: return launch_nc<64, 64, kMode>(p, stream);
-        case 96: return launch_nc<96, 32, kMode>(p, stream);
-        case 128: return p.n128 ? launch_nc<128, 128, kMode>(p, stream) : launch_nc<128, 64, kMode>(p, stream);
+        case 32: return launch_one<kMode, 32, 32>(p, stream);
+        case 64: return launch_one<kMode, 64, 64>(p, stream);
+        case 96: return launch_one<kMode, 96, 32>(p, stream);
+        case 128: return p.n128 ? launch_one<kMode, 128, 128>(p, stream) : launch_one<kMode, 128, 64>(p, stream);
         default: break;
     }
-    if constexpr (kMode != kModeRicExact) {              // split-fp16 configurations stop at 128 channels (engine.cu dsu_create)
+    if constexpr (kMode != kModeRicExact && kMode != kModeHaloExact) {              // split-fp16 configurations stop at 128 channels (engine.cu dsu_create)
         switch (p.Cout) {
-            case 160: return launch_nc<160, 32, kMode>(p, stream);
-            case 192: return launch_nc<192, 64, kMode>(p, stream);
-            case 224: return launch_nc<224, 32, kMode>(p, stream);
-            case 256: return p.n128 ? launch_nc<256, 128, kMode>(p, stream) : launch_nc<256, 64, kMode>(p, stream);
+            case 160: return launch_one<kMode, 160, 32>(p, stream);
+            case 192: return launch_one<kMode, 192, 64>(p, stream);
+            case 224: return launch_one<kMode, 224, 32>(p, stream);
+            case 256: return p.n128 ? launch_one<kMode, 256, 128>(p, stream) : launch_one<kMode, 256, 64>(p, stream);
             default: break;
         }
     }
@@ -357,7 +524,10 @@ cudaError_t launch_mode(const ConvParams& p, cudaStream_t stream) {
 
 cudaError_t launch_conv(const ConvParams& p, cudaStream_t stream) {
     if (conv_smem_bytes(p) > 227 * 1024 || p.b_bytes != p.Cout * 128) return cudaErrorInvalidConfiguration;
-    if (p.halo) return launch_mode<kModeHalo>(p, stream);
+    if (p.halo) {
+        if (p.ric || p.stride != 1 || p.up || p.ksize < 2) return cudaErrorInvalidConfiguration;
+        return p.exact ? launch_mode<kModeHaloExact>(p, stream) : launch_mode<kModeHaloFp16>(p, stream);
+    }
     if (!p.ric) return launch_mode<kModeTap>(p, stream);
     return p.exact ? launch_mode<kModeRicExact>(p, stream) : launch_mode<kModeRic>(p, stream);
 }

@@ -61,11 +61,14 @@ struct LayerDef {
     // same source pixel - exact including the zero border, 4 taps instead of 9 per output pixel.  k = 2 for such a layer and
     // wk = 3 is the kernel size of the stored weights; -1 = ordinary layer
     int sub = -1, wk = 0;
-    int first = 0;         // one <= 8-channel segment, stride 1, k > 3 (GeneratorJ.conv0): may run from a shared-memory halo
+    int pad_y = 0, pad_x = 0;  // padding above / left of the window (compiled at finalize; a sub-pixel class pads (1 - py, 1 - px))
+    int first = 0;         // one <= 8-channel segment, stride 1, k > 3 (GeneratorJ.conv0): halo mode or tap mode (knob `first`)
     // compiled at finalize
+    int halo = 0;          // chunks in halo-mode order (channel block, tap, group); the kernel reads A from a shared-memory halo
     int nchunks = 0, nblocks = 0;
     uint32_t kmask_full = 0xF, kmask_last = 0xF, kmask2_full = 0, kmask2_last = 0;
     Slot* d_slots = nullptr;
+    Slot* d_hslots = nullptr;  // halo mode: [nblocks][8] channels of each 16-byte slot of a halo pixel
     uint8_t* d_wpack = nullptr;
     float *d_scale = nullptr, *d_shift = nullptr, *d_scale2 = nullptr, *d_shift2 = nullptr;
     double macs_per_px = 0;   // live MACs per output pixel
@@ -81,6 +84,7 @@ struct Step {
 // dsu_set_knob (tests / tools).
 struct Knobs {
     int first = 1;            // the first layer builds its A chunks from a shared-memory input halo; 0 = tap mode (global loads)
+    int halo = 1;             // plan-time: the other stride-1 layers without fused upsampling and Cout <= 64 in halo mode; 0 = tap mode
     int n128 = 1;             // Cout a multiple of 128: N = 128 wgmma instructions; 0 = N = 64 (two instructions per K step)
     int subpixel = 1;         // plan-time: stage-2 nearest-x2 + 3x3 as four 2x2 sub-pixel convolutions
     int derive_edge = 0;      // stage 2, no edge map passed: burn the edges pos2edge finds in the pos frames (fused into the ingest)
@@ -88,6 +92,7 @@ struct Knobs {
 struct KnobName { const char* name; int Knobs::*field; };
 const KnobName kKnobNames[] = {
     {"first", &Knobs::first}, {"n128", &Knobs::n128}, {"subpixel", &Knobs::subpixel}, {"derive_edge", &Knobs::derive_edge},
+    {"halo", &Knobs::halo},
 };
 Knobs knobs_from_env() {
     Knobs k;
@@ -362,17 +367,19 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     // 64 K elements) holds 8 data slots (fp16 mode) or 4 data slots as [hi x4 | lo x4] (exact mode).
     // plain conv: data slots are packed densely over (tap, segment, channel group);
     // RIC conv: channel groups are packed into blocks and every block spans the 9 taps (one chunk each).
-    struct HSlot { int kh, kw, seg, choff, wch, nvalid; };
+    struct HSlot { int kh, kw, seg, choff, wch, nvalid, gi; };   // gi: channel group inside its block (halo mode)
     const int dpc = exact ? 4 : 8;            // data slots per chunk
     std::vector<std::vector<HSlot>> chunks;   // data slots of every chunk, in execution order
-    std::vector<Slot> slots;
+    std::vector<Slot> slots, hslots;
     double real_k = 0;
     for (const SegDef& s : L.segs) real_k += static_cast<double>(s.wn) * k * k;
     L.macs_per_px = real_k * C;
     // algorithmic work of a sub-pixel class = a quarter of the 3x3 layer's output pixels (flops are reported per output pixel of level_out)
     if (L.sub >= 0) L.macs_per_px = real_k / 4.0 * 9.0 / 4.0 * C;
-    // a sub-pixel class (py, px) pads its 2x2 window by (1 - py, 1 - px) above and left
-    const int pad_y = L.sub >= 0 ? 1 - (L.sub >> 1) : L.pad, pad_x = L.sub >= 0 ? 1 - (L.sub & 1) : L.pad;
+    // a sub-pixel class (py, px) pads its 2x2 window by (1 - py, 1 - px) above and left; the slot taps and the halo origin both use it
+    L.pad_y = L.sub >= 0 ? 1 - (L.sub >> 1) : L.pad;
+    L.pad_x = L.sub >= 0 ? 1 - (L.sub & 1) : L.pad;
+    const int pad_y = L.pad_y, pad_x = L.pad_x;
     auto dev_slot = [&](const HSlot& h, bool lo_plane) {
         Slot sl{};
         sl.dy = static_cast<int8_t>(h.kh - pad_y);
@@ -380,43 +387,62 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
         sl.seg = static_cast<uint8_t>(h.seg + (lo_plane ? kMaxSeg / 2 : 0));
         sl.valid = 1;
         sl.choff = static_cast<uint16_t>(h.choff);
+        sl.hslot = static_cast<uint8_t>(h.gi + (lo_plane ? 4 : 0));
         return sl;
     };
-    auto push_dev_slots = [&](const std::vector<HSlot>& ds) {
+    auto push_dev_slots = [&](const std::vector<HSlot>& ds, std::vector<Slot>& dst) {
         for (int j = 0; j < 8; ++j) {
             const int d = exact ? (j & 3) : j;
-            if (d < static_cast<int>(ds.size())) slots.push_back(dev_slot(ds[d], exact && j >= 4));
-            else slots.push_back(Slot{});
+            if (d < static_cast<int>(ds.size())) dst.push_back(dev_slot(ds[d], exact && j >= 4));
+            else dst.push_back(Slot{});
         }
     };
+    // channel groups (8 channels of one segment) over the concat, packed into blocks of one 128-byte row (RIC / halo mode)
+    std::vector<std::vector<HSlot>> blocks;
+    for (size_t si = 0; si < L.segs.size(); ++si) {
+        const SegDef& s = L.segs[si];
+        for (int c8 = 0; c8 < s.nch; c8 += 8) {
+            if (blocks.empty() || static_cast<int>(blocks.back().size()) == dpc) blocks.emplace_back();
+            blocks.back().push_back(HSlot{0, 0, (int)si, s.choff + c8, s.wch0 + c8, std::max(0, std::min(8, s.wn - c8)), (int)blocks.back().size()});
+        }
+    }
     if (!L.ric) {
         L.first = (L.stride == 1 && L.up == 0 && L.sub < 0 && L.segs.size() == 1 && L.segs[0].nch <= 8 && k > 3 && L.pad == (k - 1) / 2) ? 1 : 0;
+        // halo mode needs k >= 2: the halo of block b + 1 is loaded in the first chunk of block b and read k^2 - 1 chunks later.
+        // Only layers with Cout <= 64 (16 x 16 tiles) take it: on 8 x 16 tiles the 128-channel trunk and sub-pixel classes
+        // measured slower than tap mode (DESIGN section 7)
+        L.halo = (L.stride == 1 && L.up == 0 && k >= 2 && (L.first || (E->knobs.halo && C <= 64))) ? 1 : 0;
         std::vector<HSlot> all;
-        for (int kh = 0; kh < k; ++kh) {
-            for (int kw = 0; kw < k; ++kw)
-                for (size_t si = 0; si < L.segs.size(); ++si) {
-                    const SegDef& s = L.segs[si];
-                    for (int c8 = 0; c8 < s.nch; c8 += 8)
-                        all.push_back(HSlot{kh, kw, (int)si, s.choff + c8, s.wch0 + c8, std::max(0, std::min(8, s.wn - c8))});
-                }
+        if (L.halo) {
+            // (block, tap, group): every full block is k^2 chunks of one tap each; the last block's groups are packed densely
+            // over taps, so the chunk count equals tap mode's.  A one-group layer (conv0) gets the same chunks as in tap mode.
+            for (const std::vector<HSlot>& blk : blocks) {
+                push_dev_slots(blk, hslots);
+                for (int kh = 0; kh < k; ++kh)
+                    for (int kw = 0; kw < k; ++kw)
+                        for (HSlot h : blk) { h.kh = kh; h.kw = kw; all.push_back(h); }
+            }
+            L.nblocks = static_cast<int>(blocks.size());
+        } else {
+            for (int kh = 0; kh < k; ++kh) {
+                for (int kw = 0; kw < k; ++kw)
+                    for (size_t si = 0; si < L.segs.size(); ++si) {
+                        const SegDef& s = L.segs[si];
+                        for (int c8 = 0; c8 < s.nch; c8 += 8)
+                            all.push_back(HSlot{kh, kw, (int)si, s.choff + c8, s.wch0 + c8, std::max(0, std::min(8, s.wn - c8)), 0});
+                    }
+            }
+            L.nblocks = 0;
         }
         for (size_t i = 0; i < all.size(); i += dpc) {
             std::vector<HSlot> ds(all.begin() + i, all.begin() + std::min(all.size(), i + dpc));
-            push_dev_slots(ds);
+            push_dev_slots(ds, slots);
             chunks.push_back(ds);
         }
-        L.nblocks = 0;
     } else {
-        std::vector<HSlot> groups;            // channel groups over the concat, tap filled in per chunk
-        for (size_t si = 0; si < L.segs.size(); ++si) {
-            const SegDef& s = L.segs[si];
-            for (int c8 = 0; c8 < s.nch; c8 += 8)
-                groups.push_back(HSlot{0, 0, (int)si, s.choff + c8, s.wch0 + c8, std::max(0, std::min(8, s.wn - c8))});
-        }
-        L.nblocks = static_cast<int>((groups.size() + dpc - 1) / dpc);
-        for (int b = 0; b < L.nblocks; ++b) {
-            std::vector<HSlot> blk(groups.begin() + b * dpc, groups.begin() + std::min<size_t>(groups.size(), (b + 1) * dpc));
-            push_dev_slots(blk);                               // one slot row per BLOCK
+        L.nblocks = static_cast<int>(blocks.size());
+        for (const std::vector<HSlot>& blk : blocks) {
+            push_dev_slots(blk, slots);                        // one slot row per BLOCK
             for (int tap = 0; tap < k * k; ++tap) {
                 std::vector<HSlot> ds = blk;
                 for (HSlot& h : ds) { h.kh = tap / k; h.kw = tap % k; }
@@ -458,6 +484,7 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     L.kmask_last = hdrs.back().kmask; L.kmask2_last = hdrs.back().kmask2;
     int rc_up;
     if ((rc_up = upload(&L.d_slots, slots))) return rc_up;
+    if ((rc_up = upload(&L.d_hslots, hslots))) return rc_up;
     if ((rc_up = upload(&L.d_wpack, pack))) return rc_up;
     int rc;
 
@@ -637,6 +664,9 @@ int ensure_shape(dsu_engine* E, int B, int H, int W) {
     return DSU_OK;
 }
 
+// halo-mode plan, unless it is the first layer and knob `first` sends it to tap mode (same chunks in both orders)
+bool runs_halo(const dsu_engine* E, const LayerDef& L) { return L.halo && (!L.first || E->knobs.first != 0); }
+
 int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgba, const uint8_t* alpha_src,
                 int alpha_stride, cudaStream_t st, std::vector<cudaEvent_t>* evs = nullptr) {
     size_t step_idx = 0;
@@ -686,7 +716,9 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
         p.b_bytes = L.cout * 128;
         p.kmask_full = L.kmask_full; p.kmask_last = L.kmask_last; p.kmask2_full = L.kmask2_full; p.kmask2_last = L.kmask2_last;
         if (L.sub >= 0) { p.sub = 1; p.sub_py = L.sub >> 1; p.sub_px = L.sub & 1; }
-        p.halo = L.first && E->knobs.first != 0; p.ksize = L.k; p.pad = L.pad;
+        p.halo = runs_halo(E, L);
+        p.ksize = L.k; p.pad_y = L.pad_y; p.pad_x = L.pad_x;
+        p.hslots = L.d_hslots;
         p.n128 = E->knobs.n128 != 0;
         p.slots = L.d_slots; p.wpack = L.d_wpack;
         for (size_t i = 0; i < L.segs.size(); ++i) {
@@ -776,7 +808,7 @@ void dsu_destroy(dsu_handle h) {
     if (!h) return;
     DeviceGuard guard(h->cfg.device);
     for (LayerDef& L : h->layers) {
-        cudaFree(L.d_slots); cudaFree(L.d_wpack);
+        cudaFree(L.d_slots); cudaFree(L.d_hslots); cudaFree(L.d_wpack);
         cudaFree(L.d_scale); cudaFree(L.d_shift); cudaFree(L.d_scale2); cudaFree(L.d_shift2);
     }
     for (int b = 0; b < NBUF; ++b) { cudaFree(h->buf_hi[b]); cudaFree(h->buf_lo[b]); }
@@ -839,6 +871,8 @@ int dsu_set_knob(dsu_handle h, const char* name, int32_t value) {
         if (std::strcmp(kn.name, name) == 0) {
             if (kn.field == &Knobs::subpixel && h->knobs.subpixel != value)
                 return fail(DSU_E_STATE, "'subpixel' shapes the launch plan: set DSU_SUBPIXEL in the environment before dsu_create");
+            if (kn.field == &Knobs::halo && h->knobs.halo != value)
+                return fail(DSU_E_STATE, "'halo' shapes the weight packing: set DSU_HALO in the environment before dsu_create");
             h->knobs.*(kn.field) = value;
             return DSU_OK;
         }
@@ -994,6 +1028,14 @@ const char* dsu_step_name(dsu_handle h, int32_t index) {
     if (!h || index < 0 || index >= static_cast<int>(h->steps.size())) return "";
     const Step& sp = h->steps[index];
     return sp.type == 0 ? h->layers[sp.layer].name.c_str() : sp.type == 1 ? "maxpool" : "instance_norm";
+}
+
+const char* dsu_step_kernel(dsu_handle h, int32_t index) {
+    if (!h || index < 0 || index >= static_cast<int>(h->steps.size())) return "";
+    const Step& sp = h->steps[index];
+    if (sp.type != 0) return sp.type == 1 ? "maxpool" : "instance_norm";
+    const LayerDef& L = h->layers[sp.layer];
+    return L.ric ? "ric" : runs_halo(h, L) ? "halo" : "tap";
 }
 
 int dsu_frames_to_tensor(const uint8_t* color_dev, const uint8_t* pos_dev, const uint8_t* edge_dev,

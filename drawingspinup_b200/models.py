@@ -326,6 +326,18 @@ class _Generator(nn.Module):
             capi.check(n, "dsu_profile_forward")
         return [(capi.lib().dsu_step_name(handle, i).decode(), ms[i], fl[i]) for i in range(min(n, cap))]
 
+    def step_kernels(self):
+        """``(name, kernel)`` of every launch of the current plan (C ABI ``dsu_step_kernel``: "halo", "tap", "ric", ...);
+        valid after the first forward."""
+        lib = capi.lib()
+        out, i = [], 0
+        while True:
+            name = lib.dsu_step_name(self._handle, i).decode()
+            if not name:
+                return out
+            out.append((name, lib.dsu_step_kernel(self._handle, i).decode()))
+            i += 1
+
     def debug_buffer(self, buffer: int, plane: int, shape, dtype=torch.float16) -> torch.Tensor:
         """Test hook: host copy of an internal activation buffer (see dsu_debug_read)."""
         t = torch.empty(shape, dtype=dtype)

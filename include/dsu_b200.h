@@ -79,9 +79,9 @@ int dsu_loaded_keys(dsu_handle h);
  * tensor-core tiles, upload.  Requires every expected key (strict=True semantics). */
 int dsu_finalize(dsu_handle h, void* stream);
 
-/* Development / test hook, no counterpart in the reference: knobs of this handle ("first", "n128", "subpixel", "derive_edge" -
- * engine.cu Knobs).  Their defaults are read once from the environment (DSU_<NAME>) by dsu_create; "subpixel" shapes the launch plan
- * and can only be set through the environment (DSU_E_STATE otherwise). */
+/* Development / test hook, no counterpart in the reference: knobs of this handle ("first", "n128", "subpixel", "derive_edge",
+ * "halo" - engine.cu Knobs).  Their defaults are read once from the environment (DSU_<NAME>) by dsu_create; "subpixel" shapes the
+ * launch plan and "halo" the weight packing, so those two can only be set through the environment (DSU_E_STATE otherwise). */
 int dsu_set_knob(dsu_handle h, const char* name, int32_t value);
 
 /* generate_coordinates (models.py:551-604) is data independent; by default the engine derives the
@@ -121,6 +121,10 @@ int dsu_profile_forward(dsu_handle h, int32_t B, int32_t H, int32_t W, int32_t r
                         double* ms_out, double* flops_out, int32_t capacity);
 /* Name of launch i of a forward ("ingest", "conv0", "maxpool", "resnets.3.conv_1", ...). */
 const char* dsu_step_name(dsu_handle h, int32_t index);
+/* Mainloop launch i runs with the handle's current plan and knobs: "halo" (A fragments from a shared-memory input halo),
+ * "tap" (A tiles gathered per tap), "ric" (stage-1 deformable), or "maxpool" / "instance_norm" for the other steps.  Valid
+ * after dsu_finalize. */
+const char* dsu_step_kernel(dsu_handle h, int32_t index);
 
 /* ---- stand-alone uint8 / fp32 frame steps (device pointers) -------------------------------- */
 /* DatasetFullImages.__getitem__ (data.py:23-47): pre_dev fp32 [B,6,H,W] = RGB(3) | mask | posXY(2),
