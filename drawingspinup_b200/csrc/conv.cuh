@@ -101,6 +101,9 @@ struct ConvParams {
     int halo, ksize, pad_y, pad_x;
     const Slot* hslots;     // [nblocks][8]: the channels of each 16-byte slot of a halo pixel
     int n128;               // Cout a multiple of 128: issue N = 128 wgmma instructions (else N = 64 / 32)
+    // RIC halo mode (ric = 1): the tile's stencil entries are staged in shared memory once per CTA and the input of each
+    // channel block (the tile +- 1 pixel in source coordinates) once per block; the corners of every tap are read from there
+    int ric_halo;
 };
 
 cudaError_t launch_conv(const ConvParams& p, cudaStream_t stream);

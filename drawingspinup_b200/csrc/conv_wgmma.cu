@@ -9,7 +9,10 @@
 //   * PRODUCE chunk q + 2 while the MMAs of chunk q run.  Tap mode: each 16-byte slot of an A row is 8 channels of one
 //     tap of one concat segment (slot table), so stride 2 and fused nearest-x2 upsampling are pure address arithmetic
 //     (cp.async with zero fill at the border).  RIC (stage-1 deformable) layers blend the four bilinear corners of the
-//     rotated tap in registers and store the result.  The weight tile is streamed with cp.async.
+//     rotated tap in registers and store the result; the corners come either straight from global memory (gather
+//     producer) or, in RIC halo mode, from the channel block's input halo (the tile +- 1 source pixel, staged once per
+//     block with cp.async, double-buffered) with the tile's stencil staged once per CTA.  The weight tile is streamed
+//     with cp.async.
 //   * ISSUE wgmma: warpgroup w multiplies A rows 64w .. 64w+63 by the whole weight tile into its register accumulators.
 //
 // conv_halo_kernel (halo mode): the planner (engine.cu compile_layer) sends the first layer and every other stride-1 layer
@@ -32,11 +35,15 @@ namespace dsu {
 
 namespace {
 
-constexpr int kModeTap = 0, kModeRic = 1, kModeRicExact = 2;
+// tap mode, RIC with the gather producer, RIC with the halo producer (fp16 / split fp16)
+constexpr int kModeTap = 0, kModeRic = 1, kModeRicExact = 2, kModeRicHalo = 3, kModeRicHaloExact = 4;
 
 struct SmemLayout {
     uint32_t stage_bytes;   // A tile + B tile
-    uint32_t par;           // epilogue parameters, after the ring (the staged accumulators reuse the ring)
+    uint32_t halo;          // RIC halo mode: two input halos of halo_bytes after the ring (halo_bytes = 0 otherwise)
+    uint32_t halo_bytes;
+    uint32_t sten;          // RIC halo mode: the tile's stencil entries, [rotated tap m][tile pixel] x 8 B
+    uint32_t par;           // epilogue parameters (the staged accumulators reuse the ring, halos and stencil)
     uint32_t total;         // from the 1024-aligned base
 };
 
@@ -44,11 +51,21 @@ __host__ __device__ inline uint32_t acc_pitch(int cout) { return static_cast<uin
 
 __host__ __device__ inline uint32_t par_bytes(int cout) { return (7 * cout + 4) * 4; }
 
-__host__ __device__ inline SmemLayout smem_layout(int cout, int b_bytes) {
+// RIC halo mode: every corner of the 3 x 3 neighbourhoods of a tile lies in source rows (ty0 >> up) - 1 .. ((ty0 + kTileH) >> up)
+// and columns (tx0 >> up) - 1 .. ((tx0 + kTileW) >> up): 10 x 18 pixels at up = 0, 6 x 10 with the fused nearest x2
+__host__ __device__ inline int ric_halo_rows(int up) { return (kTileH >> up) + 2; }
+__host__ __device__ inline int ric_halo_cols(int up) { return (kTileW >> up) + 2; }
+constexpr uint32_t kStenBytes = kTileM * 8 * 8;
+
+__host__ __device__ inline SmemLayout smem_layout(int cout, int b_bytes, bool ric_halo, int up) {
     SmemLayout L;
     L.stage_bytes = kABytes + b_bytes;
     const uint32_t ring = kStages * L.stage_bytes, staged = kTileM * acc_pitch(cout) * 4;
-    L.par = ((ring > staged ? ring : staged) + 15u) & ~15u;
+    L.halo = ring;
+    L.halo_bytes = ric_halo ? static_cast<uint32_t>(ric_halo_rows(up) * ric_halo_cols(up)) * 128u : 0u;
+    L.sten = L.halo + 2 * L.halo_bytes;
+    const uint32_t main_end = L.sten + (ric_halo ? kStenBytes : 0u);
+    L.par = ((main_end > staged ? main_end : staged) + 15u) & ~15u;
     L.total = L.par + par_bytes(cout);
     return L;
 }
@@ -102,23 +119,81 @@ __device__ __forceinline__ void produce_tap(const ConvParams& p, int q, uint32_t
     }
 }
 
-// ---- RIC: chunk q = (channel block q / 9, tap q % 9).  torchvision's deform_conv2d bilinear rule with the engine's
-// stencil tables: tap t != 4 samples the 2x2 corner set of its rotated sector m at fractions (ly, lx); corners outside
-// the (virtual, nearest-x2) image read as zero.  Same operation order as the reference port of the weights:
-// w00*n00, then fma w01*n01, w10*n10, w11*n11.
+// ---- RIC: chunk q = (channel block q / 9, tap q % 9).  One A-row item = (output pixel r, data slot d).  fp16: slot d of
+// the row, 4 rows per thread; split fp16: 8 fp32 channels -> hi slot d, lo slot d + 4, 2 rows per thread.
+template <bool kExact>
+struct RicItems {
+    static constexpr int kSlots = kExact ? 4 : 8, kRowsPer = kExact ? 2 : 4, kRowStep = kTileM / kRowsPer;
+};
+
+// torchvision's deform_conv2d bilinear rule with the engine's stencil tables: the centre tap copies corner (0, 0); a rotated
+// tap blends the 2x2 corner set of its sector with the stencil entry `entry()` (fp16: the four fp16 weights {w00,w01 | w10,w11};
+// split fp16: the fractions (ly, lx)), in the operation order of the reference port of the weights: w00*n00, then fma w01*n01,
+// w10*n10, w11*n11.  `fetch(cy, cx, h)` returns 16 source bytes of corner (cy, cx), zeros outside the (virtual, nearest-x2)
+// image: the 8 fp16 channels (h = 0), or fp32 channels 4h .. 4h + 3.  Both RIC producers go through here and differ only in
+// `entry` and `fetch`, so they write bit-identical A rows.
+template <bool kExact, typename Entry, typename Fetch>
+__device__ __forceinline__ void ric_item(bool centre, const Entry& entry, const Fetch& fetch, uint32_t row, int d, uint32_t swz) {
+    if constexpr (!kExact) {
+        uint4 out;
+        if (centre) {
+            out = fetch(0, 0, 0);
+        } else {
+            const uint2 wv = entry();
+            const __half2 wa = *reinterpret_cast<const __half2*>(&wv.x), wb = *reinterpret_cast<const __half2*>(&wv.y);
+            const __half2 w00 = __low2half2(wa), w01 = __high2half2(wa), w10 = __low2half2(wb), w11 = __high2half2(wb);
+            const uint4 n00 = fetch(0, 0, 0), n01 = fetch(0, 1, 0), n10 = fetch(1, 0, 0), n11 = fetch(1, 1, 0);
+            const __half2* h00 = reinterpret_cast<const __half2*>(&n00);
+            const __half2* h01 = reinterpret_cast<const __half2*>(&n01);
+            const __half2* h10 = reinterpret_cast<const __half2*>(&n10);
+            const __half2* h11 = reinterpret_cast<const __half2*>(&n11);
+            __half2* o = reinterpret_cast<__half2*>(&out);
+#pragma unroll
+            for (int c = 0; c < 4; ++c) o[c] = __hfma2(w11, h11[c], __hfma2(w10, h10[c], __hfma2(w01, h01[c], __hmul2(w00, h00[c]))));
+        }
+        st_shared_v4(row + ((static_cast<uint32_t>(d) ^ swz) << 4), out);
+    } else {
+        // split-fp16 stage 1 keeps fp32 activations: 8 channels = two 16-byte fetches per corner
+        auto load8 = [&](int cy, int cx, float* v) {
+            const uint4 lo = fetch(cy, cx, 0), hi = fetch(cy, cx, 1);
+            v[0] = __uint_as_float(lo.x); v[1] = __uint_as_float(lo.y); v[2] = __uint_as_float(lo.z); v[3] = __uint_as_float(lo.w);
+            v[4] = __uint_as_float(hi.x); v[5] = __uint_as_float(hi.y); v[6] = __uint_as_float(hi.z); v[7] = __uint_as_float(hi.w);
+        };
+        float f[8];
+        if (centre) {
+            load8(0, 0, f);
+        } else {
+            const float2 l = entry();
+            const float hy = 1.0f - l.x, hx = 1.0f - l.y;
+            const float w0 = __fmul_rn(hy, hx), w1 = __fmul_rn(hy, l.y), w2 = __fmul_rn(l.x, hx), w3 = __fmul_rn(l.x, l.y);
+            float v00[8], v01[8], v10[8], v11[8];
+            load8(0, 0, v00); load8(0, 1, v01); load8(1, 0, v10); load8(1, 1, v11);
+#pragma unroll
+            for (int c = 0; c < 8; ++c) f[c] = __fmaf_rn(w3, v11[c], __fmaf_rn(w2, v10[c], __fmaf_rn(w1, v01[c], __fmul_rn(w0, v00[c]))));
+        }
+        uint4 hi, lo;
+        split8(f, hi, lo);
+        st_shared_v4(row + ((static_cast<uint32_t>(d) ^ swz) << 4), hi);
+        st_shared_v4(row + ((static_cast<uint32_t>(d + 4) ^ swz) << 4), lo);
+    }
+}
+
+// ---- RIC gather producer: octant, stencil entry and the four corners of every item straight from L2 / global memory
 template <bool kExact>
 __device__ __forceinline__ void produce_ric(const ConvParams& p, int q, uint32_t a, int tid, int n, int ty0, int tx0) {
+    using It = RicItems<kExact>;
     const int blk = q / 9, t = q - 9 * blk;
     const int kq = t < 4 ? t : t - 1;                     // circle index of a rotated tap
     const size_t frame_in = static_cast<size_t>(n) * p.Hin * p.Win;
-    // fp16: one item = (row, slot j), 4 rows per thread; split-fp16: one item = (row, data slot d) -> hi slot d, lo slot d + 4
-    constexpr int kSlots = kExact ? 4 : 8, kRowsPer = kExact ? 2 : 4, kRowStep = kTileM / kRowsPer;
-    const int d = tid % kSlots, prow = tid / kSlots;
+    const int d = tid % It::kSlots, prow = tid / It::kSlots;
     const Slot sl = p.slots[blk * 8 + d];
     const Seg sg = p.seg[sl.seg];
+    constexpr size_t kEsz = kExact ? sizeof(float) : sizeof(__half);
+    const uint8_t* src = reinterpret_cast<const uint8_t*>(sg.ptr) + sl.choff * kEsz;
+    const size_t pitch = static_cast<size_t>(sg.pitch) * kEsz;
 #pragma unroll
-    for (int i = 0; i < kRowsPer; ++i) {
-        const int r = prow + kRowStep * i;
+    for (int i = 0; i < It::kRowsPer; ++i) {
+        const int r = prow + It::kRowStep * i;
         const int oy = ty0 + (r >> 4), ox = tx0 + (r & 15);
         const bool live = sl.valid && oy < p.Hout && ox < p.Wout;
         const size_t e = live ? static_cast<size_t>(oy) * p.Wout + ox : 0;
@@ -127,67 +202,114 @@ __device__ __forceinline__ void produce_ric(const ConvParams& p, int q, uint32_t
             m = (kq + __ldg(p.ric_oct + e)) & 7;
             dy0 = ric_r0(m) - 1; dx0 = ric_c0(m) - 1;
         }
-        // corner (cy, cx) of the sample -> pointer into the source (null when outside the image)
-        auto corner = [&](int cy, int cx, bool& ok) {
+        auto fetch = [&](int cy, int cx, int h) {
             const int vy = oy + dy0 + cy, vx = ox + dx0 + cx;
-            ok = live && static_cast<unsigned>(vy) < static_cast<unsigned>(p.Hv) && static_cast<unsigned>(vx) < static_cast<unsigned>(p.Wv);
-            return ok ? frame_in + static_cast<size_t>(vy >> p.up) * p.Win + (vx >> p.up) : 0;
+            const bool ok = live && static_cast<unsigned>(vy) < static_cast<unsigned>(p.Hv) && static_cast<unsigned>(vx) < static_cast<unsigned>(p.Wv);
+            const size_t pix = ok ? frame_in + static_cast<size_t>(vy >> p.up) * p.Win + (vx >> p.up) : 0;
+            return ldg128_if(src + pix * pitch + 16 * h, ok);
         };
-        const uint32_t row = a + static_cast<uint32_t>(r) * 128u;
-        const uint32_t swz = static_cast<uint32_t>(r & 7);
-        if constexpr (!kExact) {
-            const __half* src = sg.ptr + sl.choff;
-            uint4 out;
-            if (t == 4) {
-                bool ok;
-                const size_t pix = corner(0, 0, ok);
-                out = ldg128_if(src + pix * sg.pitch, ok);
-            } else {
-                const uint2 wv = live ? __ldg(p.ric_wh + e * 8 + m) : make_uint2(0u, 0u);
-                const __half2 wa = *reinterpret_cast<const __half2*>(&wv.x), wb = *reinterpret_cast<const __half2*>(&wv.y);
-                const __half2 w00 = __low2half2(wa), w01 = __high2half2(wa), w10 = __low2half2(wb), w11 = __high2half2(wb);
-                bool k00, k01, k10, k11;
-                const size_t p00 = corner(0, 0, k00), p01 = corner(0, 1, k01), p10 = corner(1, 0, k10), p11 = corner(1, 1, k11);
-                const uint4 n00 = ldg128_if(src + p00 * sg.pitch, k00), n01 = ldg128_if(src + p01 * sg.pitch, k01);
-                const uint4 n10 = ldg128_if(src + p10 * sg.pitch, k10), n11 = ldg128_if(src + p11 * sg.pitch, k11);
-                const __half2* h00 = reinterpret_cast<const __half2*>(&n00);
-                const __half2* h01 = reinterpret_cast<const __half2*>(&n01);
-                const __half2* h10 = reinterpret_cast<const __half2*>(&n10);
-                const __half2* h11 = reinterpret_cast<const __half2*>(&n11);
-                __half2* o = reinterpret_cast<__half2*>(&out);
+        auto entry = [&]() {
+            if constexpr (kExact) return live ? __ldg(p.ric_lyx + e * 8 + m) : make_float2(0.0f, 0.0f);
+            else return live ? __ldg(p.ric_wh + e * 8 + m) : make_uint2(0u, 0u);
+        };
+        ric_item<kExact>(t == 4, entry, fetch, a + static_cast<uint32_t>(r) * 128u, d, static_cast<uint32_t>(r & 7));
+    }
+}
+
+// ---- RIC halo mode: what a CTA stages once, and the per-thread octants of its items (byte i = item row i)
+struct RicTile {
+    uint32_t halo, halo_bytes;  // two input-halo buffers: block b in buffer b & 1
+    uint32_t sten;              // stencil entries [m][pixel], 8 B each
+    uint32_t oct;
+};
+
+// The stencil entries of the tile's 128 pixels (fp16 weights or split-fp16 fractions: 8 B per rotated tap), stored
+// [m][pixel] so that the items of one load phase (neighbouring pixels, any sectors) hit distinct banks; zeros outside
+// Hout x Wout.  The octants go to registers: an item's output pixel never changes across chunks.  (They are read with
+// plain loads: a tile row of octant bytes is not 4-byte aligned when Wout is not a multiple of 4.)
+template <bool kExact>
+__device__ __forceinline__ uint32_t load_ric_stencil(const ConvParams& p, uint32_t sten, int tid, int ty0, int tx0) {
+    using It = RicItems<kExact>;
+    const uint8_t* table = kExact ? reinterpret_cast<const uint8_t*>(p.ric_lyx) : reinterpret_cast<const uint8_t*>(p.ric_wh);
+    for (int i = tid; i < kTileM * 8; i += kThreads) {
+        const int r = i >> 3, m = i & 7;
+        const int oy = ty0 + (r >> 4), ox = tx0 + (r & 15);
+        const bool ok = oy < p.Hout && ox < p.Wout;
+        const size_t e = ok ? static_cast<size_t>(oy) * p.Wout + ox : 0;
+        cp_async8(sten + static_cast<uint32_t>(m * kTileM + r) * 8u, table + (e * 8 + m) * 8, ok ? 8u : 0u);
+    }
+    uint32_t oct = 0;
 #pragma unroll
-                for (int c = 0; c < 4; ++c) o[c] = __hfma2(w11, h11[c], __hfma2(w10, h10[c], __hfma2(w01, h01[c], __hmul2(w00, h00[c]))));
-            }
-            st_shared_v4(row + ((static_cast<uint32_t>(d) ^ swz) << 4), out);
-        } else {
-            // split-fp16 stage 1 keeps fp32 activations: 8 channels = two 16-byte loads per corner
-            const float* src = reinterpret_cast<const float*>(sg.ptr) + sl.choff;
-            float f[8];
-            auto load8 = [&](size_t pix, bool ok, float* v) {
-                const uint4 lo = ldg128_if(src + pix * sg.pitch, ok), hi = ldg128_if(src + pix * sg.pitch + 4, ok);
-                v[0] = __uint_as_float(lo.x); v[1] = __uint_as_float(lo.y); v[2] = __uint_as_float(lo.z); v[3] = __uint_as_float(lo.w);
-                v[4] = __uint_as_float(hi.x); v[5] = __uint_as_float(hi.y); v[6] = __uint_as_float(hi.z); v[7] = __uint_as_float(hi.w);
-            };
-            if (t == 4) {
-                bool ok;
-                const size_t pix = corner(0, 0, ok);
-                load8(pix, ok, f);
-            } else {
-                const float2 l = live ? __ldg(p.ric_lyx + e * 8 + m) : make_float2(0.0f, 0.0f);
-                const float hy = 1.0f - l.x, hx = 1.0f - l.y;
-                const float w0 = __fmul_rn(hy, hx), w1 = __fmul_rn(hy, l.y), w2 = __fmul_rn(l.x, hx), w3 = __fmul_rn(l.x, l.y);
-                bool k00, k01, k10, k11;
-                const size_t p00 = corner(0, 0, k00), p01 = corner(0, 1, k01), p10 = corner(1, 0, k10), p11 = corner(1, 1, k11);
-                float v00[8], v01[8], v10[8], v11[8];
-                load8(p00, k00, v00); load8(p01, k01, v01); load8(p10, k10, v10); load8(p11, k11, v11);
+    for (int i = 0; i < It::kRowsPer; ++i) {
+        const int r = tid / It::kSlots + It::kRowStep * i;
+        const int oy = ty0 + (r >> 4), ox = tx0 + (r & 15);
+        if (oy < p.Hout && ox < p.Wout) oct |= static_cast<uint32_t>(__ldg(p.ric_oct + static_cast<size_t>(oy) * p.Wout + ox)) << (8 * i);
+    }
+    return oct;
+}
+
+// The input of channel block `blk` for the whole tile: source rows (ty0 >> up) - 1 + [0, ric_halo_rows), columns
+// (tx0 >> up) - 1 + [0, ric_halo_cols), 128 B per pixel, pixel-major, 16-byte slot s at ((s ^ (pixel & 7)) << 4).  Slot s
+// holds group s (fp16) or half s & 1 of group s / 2 (fp32: channels 4 (s & 1) .. + 3) of the block's RIC slot table.
+// Zeros outside [0, Hin) x [0, Win) (torchvision's border rule: corners outside the virtual image read zero) and for
+// K-padding slots.
+template <bool kExact>
+__device__ __forceinline__ void load_ric_halo(const ConvParams& p, int blk, uint32_t halo, int tid, int n, int ty0, int tx0) {
+    const int hw = ric_halo_cols(p.up), npix = ric_halo_rows(p.up) * hw;
+    const int y0 = (ty0 >> p.up) - 1, x0 = (tx0 >> p.up) - 1;
+    const int s = tid & 7;                                // the 8 threads of a pixel copy its 128 bytes
+    const Slot sl = p.slots[blk * 8 + (kExact ? s >> 1 : s)];
+    const Seg sg = p.seg[sl.seg];
+    constexpr size_t kEsz = kExact ? sizeof(float) : sizeof(__half);
+    const uint8_t* sbase = reinterpret_cast<const uint8_t*>(sg.ptr) + (sl.choff + (kExact ? 4 * (s & 1) : 0)) * kEsz;
+    const size_t pitch = static_cast<size_t>(sg.pitch) * kEsz;
+    const size_t frame_in = static_cast<size_t>(n) * p.Hin * p.Win;
+    for (int pix = tid >> 3; pix < npix; pix += kThreads / 8) {
+        const int hy = pix / hw, hx = pix - hy * hw;
+        const int y = y0 + hy, x = x0 + hx;
+        const bool ok = sl.valid && static_cast<unsigned>(y) < static_cast<unsigned>(p.Hin) && static_cast<unsigned>(x) < static_cast<unsigned>(p.Win);
+        const uint8_t* src = ok ? sbase + (frame_in + static_cast<size_t>(y) * p.Win + x) * pitch : sbase;
+        cp_async16(halo + static_cast<uint32_t>(pix) * 128u + (static_cast<uint32_t>(s ^ (pix & 7)) << 4), src, ok ? 16u : 0u);
+    }
+}
+
+// ---- RIC halo producer: the gather producer's items with the stencil entry from shared memory and the corners from the
+// block's halo.  A corner (vy, vx) of the virtual image is halo pixel ((vy >> up) - y0, (vx >> up) - x0); rows and columns past
+// Hout / Wout in ragged tiles stay inside the halo and produce zeros (`live`).  Bank conflicts: a load phase of 8 threads is
+// one pixel's 8 slots (fp16), or 2 horizontally adjacent pixels x 4 groups (split fp16) whose corners of one sector are
+// adjacent halo pixels, i.e. swizzle keys differing in bit 0: disjoint bank quads (2-way only where the two pixels' sectors
+// differ).  Stencil reads are broadcasts within a pixel and consecutive 8-byte words across pixels.
+template <bool kExact>
+__device__ __forceinline__ void produce_ric_halo(const ConvParams& p, int q, uint32_t a, int tid, int ty0, int tx0, const RicTile& rt) {
+    using It = RicItems<kExact>;
+    const int blk = q / 9, t = q - 9 * blk;
+    const int kq = t < 4 ? t : t - 1;
+    const int d = tid % It::kSlots, prow = tid / It::kSlots;
+    const bool valid = p.slots[blk * 8 + d].valid;
+    const uint32_t halo = rt.halo + static_cast<uint32_t>(blk & 1) * rt.halo_bytes;
+    const int hw = ric_halo_cols(p.up), y0 = (ty0 >> p.up) - 1, x0 = (tx0 >> p.up) - 1;
 #pragma unroll
-                for (int c = 0; c < 8; ++c) f[c] = __fmaf_rn(w3, v11[c], __fmaf_rn(w2, v10[c], __fmaf_rn(w1, v01[c], __fmul_rn(w0, v00[c]))));
-            }
-            uint4 hi, lo;
-            split8(f, hi, lo);
-            st_shared_v4(row + ((static_cast<uint32_t>(d) ^ swz) << 4), hi);
-            st_shared_v4(row + ((static_cast<uint32_t>(d + 4) ^ swz) << 4), lo);
+    for (int i = 0; i < It::kRowsPer; ++i) {
+        const int r = prow + It::kRowStep * i;
+        const int oy = ty0 + (r >> 4), ox = tx0 + (r & 15);
+        const bool live = valid && oy < p.Hout && ox < p.Wout;
+        int dy0 = 0, dx0 = 0, m = 0;
+        if (t != 4) {
+            m = (kq + (rt.oct >> (8 * i))) & 7;
+            dy0 = ric_r0(m) - 1; dx0 = ric_c0(m) - 1;
         }
+        auto fetch = [&](int cy, int cx, int h) {
+            const int hp = (((oy + dy0 + cy) >> p.up) - y0) * hw + ((ox + dx0 + cx) >> p.up) - x0;
+            const uint32_t s = kExact ? static_cast<uint32_t>(2 * d + h) : static_cast<uint32_t>(d);
+            const uint4 v = ld_shared_v4(halo + static_cast<uint32_t>(hp) * 128u + ((s ^ static_cast<uint32_t>(hp & 7)) << 4));
+            return live ? v : make_uint4(0u, 0u, 0u, 0u);
+        };
+        auto entry = [&]() {
+            const uint2 raw = ld_shared_v2(rt.sten + static_cast<uint32_t>(m * kTileM + r) * 8u);
+            if constexpr (kExact) return make_float2(__uint_as_float(raw.x), __uint_as_float(raw.y));
+            else return raw;
+        };
+        ric_item<kExact>(t == 4, entry, fetch, a + static_cast<uint32_t>(r) * 128u, d, static_cast<uint32_t>(r & 7));
     }
 }
 
@@ -197,10 +319,20 @@ __device__ __forceinline__ void produce_b(const ConvParams& p, int q, uint32_t d
     for (int i = tid; i < p.b_bytes / 16; i += kThreads) cp_async16(dst + 16u * i, src + 16 * i, 16u);
 }
 
+// chunk q: A rows and weight tile; in RIC halo mode the first chunk of block b also starts the halo of block b + 1
 template <int kMode>
-__device__ __forceinline__ void produce(const ConvParams& p, int q, uint32_t stage, int tid, int n, int ty0, int tx0) {
-    if constexpr (kMode == kModeTap) produce_tap(p, q, stage, tid, n, ty0, tx0);
-    else produce_ric<kMode == kModeRicExact>(p, q, stage, tid, n, ty0, tx0);
+__device__ __forceinline__ void produce(const ConvParams& p, int q, uint32_t stage, int tid, int n, int ty0, int tx0, const RicTile& rt) {
+    if constexpr (kMode == kModeTap) {
+        produce_tap(p, q, stage, tid, n, ty0, tx0);
+    } else if constexpr (kMode == kModeRic || kMode == kModeRicExact) {
+        produce_ric<kMode == kModeRicExact>(p, q, stage, tid, n, ty0, tx0);
+    } else {
+        constexpr bool kExact = kMode == kModeRicHaloExact;
+        const int blk = q / 9;
+        if (q == 9 * blk && blk + 1 < p.nblocks)
+            load_ric_halo<kExact>(p, blk + 1, rt.halo + static_cast<uint32_t>((blk + 1) & 1) * rt.halo_bytes, tid, n, ty0, tx0);
+        produce_ric_halo<kExact>(p, q, stage, tid, ty0, tx0, rt);
+    }
     produce_b(p, q, stage + kABytes, tid);
 }
 
@@ -320,14 +452,23 @@ __device__ __forceinline__ void store_tile(const ConvParams& p, uint8_t* smem, c
 }  // namespace
 
 // NC = Cout, PN = wgmma N per instruction (a divisor of NC: 32, 64 or 128)
+//
+// RIC halo mode: the prologue stages the tile's stencil and the halo of channel block 0 (one cp.async group, waited for and
+// made visible by a barrier before chunk 0 is produced).  Producers run two chunks ahead: chunk c is produced in iteration
+// c - 2 (chunks 0 and 1 in the prologue), so the first chunk of block b (c = 9b) is produced in iteration 9b - 2, and the
+// halo of block b + 1 is issued there, in that iteration's cp.async group.  Block b + 1 is first read by chunk 9b + 9, produced
+// in iteration 9b + 7, whose cp_async_wait<kStages - 3> (every group but the newest, i.e. up to iteration 9b + 5's) and
+// barrier make it visible.  It overwrites the buffer of block b - 1, whose last chunk 9b - 1 was produced in iteration 9b - 3,
+// before the barrier of iteration 9b - 2.
 template <int NC, int PN, int kMode>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
+    constexpr bool kRicHalo = kMode == kModeRicHalo || kMode == kModeRicHaloExact;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_u32 = smem_u32(smem_raw);
     const uint32_t base = (raw_u32 + 1023u) & ~1023u;     // SWIZZLE_128B atoms are 1024-byte aligned
     uint8_t* smem = smem_raw + (base - raw_u32);
-    const SmemLayout L = smem_layout(NC, p.b_bytes);
+    const SmemLayout L = smem_layout(NC, p.b_bytes, kRicHalo, p.up);
     float* s_par = reinterpret_cast<float*>(smem + L.par);
 
     const int tid = threadIdx.x;
@@ -337,7 +478,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     const int tx0 = blockIdx.x * kTileW;
     const int nq = p.nchunks;
     // chunks with the ragged K tail: the last one (tap mode) or the 9 taps of the last channel block (RIC)
-    const int tail_from = (kMode == kModeRic || kMode == kModeRicExact) ? (p.nblocks - 1) * 9 : nq - 1;
+    const int tail_from = kMode != kModeTap ? (p.nblocks - 1) * 9 : nq - 1;
 
     load_epilogue_params(p, s_par, tid, kThreads);
 
@@ -345,10 +486,19 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
 #pragma unroll
     for (int i = 0; i < NC / 2; ++i) acc[0][i] = 0.0f;
 
+    RicTile rt{base + L.halo, L.halo_bytes, base + L.sten, 0u};
+    if constexpr (kRicHalo) {
+        constexpr bool kExact = kMode == kModeRicHaloExact;
+        rt.oct = load_ric_stencil<kExact>(p, rt.sten, tid, ty0, tx0);
+        load_ric_halo<kExact>(p, 0, rt.halo, tid, n, ty0, tx0);
+        cp_async_commit();
+        cp_async_wait<0>();
+        __syncthreads();                                  // stencil and halo 0 visible to every thread
+    }
     // prologue: chunks 0 and 1; every iteration commits one cp.async group so that "chunk q has landed" is wait_group 1
 #pragma unroll
     for (int s = 0; s < kStages - 2; ++s) {
-        if (s < nq) produce<kMode>(p, s, base + s * L.stage_bytes, tid, n, ty0, tx0);
+        if (s < nq) produce<kMode>(p, s, base + s * L.stage_bytes, tid, n, ty0, tx0, rt);
         cp_async_commit();
     }
     for (int q = 0; q < nq; ++q) {
@@ -362,7 +512,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
         mma_chunk<NC, PN>(acc[0], da, db, tail ? p.kmask_last : p.kmask_full, tail ? p.kmask2_last : p.kmask2_full);
         wgmma_commit();
         wgmma_wait<1>();                                  // this warpgroup's MMAs of chunk q - 1 have retired
-        if (q + kStages - 2 < nq) produce<kMode>(p, q + kStages - 2, base + ((q + kStages - 2) % kStages) * L.stage_bytes, tid, n, ty0, tx0);
+        if (q + kStages - 2 < nq) produce<kMode>(p, q + kStages - 2, base + ((q + kStages - 2) % kStages) * L.stage_bytes, tid, n, ty0, tx0, rt);
         cp_async_commit();
     }
     wgmma_wait<0>();
@@ -451,7 +601,8 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
 }
 
 size_t conv_smem_bytes(const ConvParams& p) {
-    const uint32_t total = p.halo ? halo_layout(p.Cout, halo_rows(p.Cout), p.ksize).total : smem_layout(p.Cout, p.b_bytes).total;
+    const uint32_t total = p.halo ? halo_layout(p.Cout, halo_rows(p.Cout), p.ksize).total
+                                  : smem_layout(p.Cout, p.b_bytes, p.ric && p.ric_halo, p.up).total;
     return total + 1024;
 }
 
@@ -490,8 +641,8 @@ cudaError_t launch_halo_nc(const ConvParams& p, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
-// halo mode in fp16 / split fp16 (same numbering as the tap / RIC modes of launch_nc)
-constexpr int kModeHaloFp16 = 3, kModeHaloExact = 4;
+// halo mode in fp16 / split fp16 (numbered after the tap / RIC modes of launch_nc)
+constexpr int kModeHaloFp16 = 5, kModeHaloExact = 6;
 
 template <int kMode, int NC, int PN>
 cudaError_t launch_one(const ConvParams& p, cudaStream_t stream) {
@@ -508,7 +659,7 @@ cudaError_t launch_mode(const ConvParams& p, cudaStream_t stream) {
         case 128: return p.n128 ? launch_one<kMode, 128, 128>(p, stream) : launch_one<kMode, 128, 64>(p, stream);
         default: break;
     }
-    if constexpr (kMode != kModeRicExact && kMode != kModeHaloExact) {              // split-fp16 configurations stop at 128 channels (engine.cu dsu_create)
+    if constexpr (kMode != kModeRicExact && kMode != kModeRicHaloExact && kMode != kModeHaloExact) {              // split-fp16 configurations stop at 128 channels (engine.cu dsu_create)
         switch (p.Cout) {
             case 160: return launch_one<kMode, 160, 32>(p, stream);
             case 192: return launch_one<kMode, 192, 64>(p, stream);
@@ -528,7 +679,9 @@ cudaError_t launch_conv(const ConvParams& p, cudaStream_t stream) {
         if (p.ric || p.stride != 1 || p.up || p.ksize < 2) return cudaErrorInvalidConfiguration;
         return p.exact ? launch_mode<kModeHaloExact>(p, stream) : launch_mode<kModeHaloFp16>(p, stream);
     }
-    if (!p.ric) return launch_mode<kModeTap>(p, stream);
+    if (!p.ric) return p.ric_halo ? cudaErrorInvalidConfiguration : launch_mode<kModeTap>(p, stream);
+    if (p.stride != 1 || p.ksize != 3) return cudaErrorInvalidConfiguration;
+    if (p.ric_halo) return p.exact ? launch_mode<kModeRicHaloExact>(p, stream) : launch_mode<kModeRicHalo>(p, stream);
     return p.exact ? launch_mode<kModeRicExact>(p, stream) : launch_mode<kModeRic>(p, stream);
 }
 

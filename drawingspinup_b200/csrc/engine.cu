@@ -88,11 +88,12 @@ struct Knobs {
     int n128 = 1;             // Cout a multiple of 128: N = 128 wgmma instructions; 0 = N = 64 (two instructions per K step)
     int subpixel = 1;         // plan-time: stage-2 nearest-x2 + 3x3 as four 2x2 sub-pixel convolutions
     int derive_edge = 0;      // stage 2, no edge map passed: burn the edges pos2edge finds in the pos frames (fused into the ingest)
+    int ric_halo = 1;         // RIC layers whose shared-memory layout fits read stencil and corners from shared memory; 0 = gather
 };
 struct KnobName { const char* name; int Knobs::*field; };
 const KnobName kKnobNames[] = {
     {"first", &Knobs::first}, {"n128", &Knobs::n128}, {"subpixel", &Knobs::subpixel}, {"derive_edge", &Knobs::derive_edge},
-    {"halo", &Knobs::halo},
+    {"halo", &Knobs::halo}, {"ric_halo", &Knobs::ric_halo},
 };
 Knobs knobs_from_env() {
     Knobs k;
@@ -667,6 +668,16 @@ int ensure_shape(dsu_engine* E, int B, int H, int W) {
 // halo-mode plan, unless it is the first layer and knob `first` sends it to tap mode (same chunks in both orders)
 bool runs_halo(const dsu_engine* E, const LayerDef& L) { return L.halo && (!L.first || E->knobs.first != 0); }
 
+// RIC layer with the halo producer: knob `ric_halo` on and the layout (ring, two input halos, stencil, epilogue parameters)
+// fits 227 KB.  Every split-fp16 width (Cout <= 128) fits; in fp16, Cout >= 224 without fused upsampling (18-column halos)
+// does not and keeps the gather producer.  Same chunks and weight packing either way, so the knob may change at run time.
+bool runs_ric_halo(const dsu_engine* E, const LayerDef& L) {
+    if (!L.ric || !E->knobs.ric_halo) return false;
+    ConvParams p{};
+    p.Cout = L.cout; p.b_bytes = L.cout * 128; p.up = L.up; p.ric = 1; p.ric_halo = 1;
+    return conv_smem_bytes(p) <= 227 * 1024;
+}
+
 int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgba, const uint8_t* alpha_src,
                 int alpha_stride, cudaStream_t st, std::vector<cudaEvent_t>* evs = nullptr) {
     size_t step_idx = 0;
@@ -720,6 +731,7 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
         p.ksize = L.k; p.pad_y = L.pad_y; p.pad_x = L.pad_x;
         p.hslots = L.d_hslots;
         p.n128 = E->knobs.n128 != 0;
+        p.ric_halo = runs_ric_halo(E, L);
         p.slots = L.d_slots; p.wpack = L.d_wpack;
         for (size_t i = 0; i < L.segs.size(); ++i) {
             p.seg[i].ptr = E->buf_hi[L.segs[i].buf];
@@ -1035,7 +1047,8 @@ const char* dsu_step_kernel(dsu_handle h, int32_t index) {
     const Step& sp = h->steps[index];
     if (sp.type != 0) return sp.type == 1 ? "maxpool" : "instance_norm";
     const LayerDef& L = h->layers[sp.layer];
-    return L.ric ? "ric" : runs_halo(h, L) ? "halo" : "tap";
+    if (L.ric) return runs_ric_halo(h, L) ? "ric_halo" : "ric";
+    return runs_halo(h, L) ? "halo" : "tap";
 }
 
 int dsu_frames_to_tensor(const uint8_t* color_dev, const uint8_t* pos_dev, const uint8_t* edge_dev,

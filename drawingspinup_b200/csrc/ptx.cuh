@@ -15,6 +15,10 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
+// 8-byte form (LDGSTS.64, through L1: the 16-byte .cg form has no 8-byte size)
+__device__ __forceinline__ void cp_async8(uint32_t dst, const void* src, uint32_t src_bytes) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
@@ -22,6 +26,11 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
     uint4 v;
     asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint2 ld_shared_v2(uint32_t addr) {
+    uint2 v;
+    asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr) : "memory");
     return v;
 }
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint4& v) {

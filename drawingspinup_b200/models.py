@@ -327,7 +327,8 @@ class _Generator(nn.Module):
         return [(capi.lib().dsu_step_name(handle, i).decode(), ms[i], fl[i]) for i in range(min(n, cap))]
 
     def step_kernels(self):
-        """``(name, kernel)`` of every launch of the current plan (C ABI ``dsu_step_kernel``: "halo", "tap", "ric", ...);
+        """``(name, kernel)`` of every launch of the current plan (C ABI ``dsu_step_kernel``: "halo", "tap", "ric_halo"
+        (stage-1 RIC with stencil and input staged in shared memory), "ric" (stage-1 RIC gathering from global memory), ...);
         valid after the first forward."""
         lib = capi.lib()
         out, i = [], 0

@@ -80,7 +80,7 @@ int dsu_loaded_keys(dsu_handle h);
 int dsu_finalize(dsu_handle h, void* stream);
 
 /* Development / test hook, no counterpart in the reference: knobs of this handle ("first", "n128", "subpixel", "derive_edge",
- * "halo" - engine.cu Knobs).  Their defaults are read once from the environment (DSU_<NAME>) by dsu_create; "subpixel" shapes the
+ * "halo", "ric_halo" - engine.cu Knobs).  Their defaults are read once from the environment (DSU_<NAME>) by dsu_create; "subpixel" shapes the
  * launch plan and "halo" the weight packing, so those two can only be set through the environment (DSU_E_STATE otherwise). */
 int dsu_set_knob(dsu_handle h, const char* name, int32_t value);
 
@@ -122,8 +122,8 @@ int dsu_profile_forward(dsu_handle h, int32_t B, int32_t H, int32_t W, int32_t r
 /* Name of launch i of a forward ("ingest", "conv0", "maxpool", "resnets.3.conv_1", ...). */
 const char* dsu_step_name(dsu_handle h, int32_t index);
 /* Mainloop launch i runs with the handle's current plan and knobs: "halo" (A fragments from a shared-memory input halo),
- * "tap" (A tiles gathered per tap), "ric" (stage-1 deformable), or "maxpool" / "instance_norm" for the other steps.  Valid
- * after dsu_finalize. */
+ * "tap" (A tiles gathered per tap), "ric_halo" (stage-1 deformable, stencil and corners from shared memory), "ric" (stage-1
+ * deformable, gathered from global memory), or "maxpool" / "instance_norm" for the other steps.  Valid after dsu_finalize. */
 const char* dsu_step_kernel(dsu_handle h, int32_t index);
 
 /* ---- stand-alone uint8 / fp32 frame steps (device pointers) -------------------------------- */
