@@ -16,6 +16,21 @@ constexpr int kThreads = 256;   // two warpgroups: producers, MMA issuers and ep
 constexpr int kStages = 4;      // A + B ring depth; chunk q + 2 is loaded while the MMAs of chunk q run
 constexpr int kMaxSeg = 6;      // concat segments (second half = lo planes in exact mode)
 
+// Which mainloop and A producer a convolution launch runs.  This is the one statement of the rule (engine.cu compile_layer
+// records the plan-time mode, conv_mode applies the run-time knobs):
+//   * stage-1 (RIC) layers run RicHalo where its shared-memory layout fits 227 KB (every split-fp16 layer; in fp16 not Cout >= 224
+//     without fused upsampling), else Ric.  Knob `ric_halo` = 0 keeps them all on Ric.
+//   * a stage-2 layer runs Halo when it is stride 1 without fused upsampling and either conv0-shaped or Cout <= 64 (wider layers
+//     measured slower on 8 x 16 halo tiles, DESIGN section 7); plan-time knob `halo` (DSU_HALO) = 0 keeps all but conv0 on
+//     Tap, and run-time knob `first` = 0 sends conv0 to Tap.  Every other layer runs Tap.
+// The run-time alternatives use the same chunks and weight packing as the plan-time mode.
+enum class ConvMode : int {
+    Tap,        // conv_wgmma_kernel: each A slot gathered from global memory per (chunk, slot) with cp.async
+    Ric,        // conv_wgmma_kernel: stage-1 deformable, the bilinear corners gathered from global memory
+    RicHalo,    // conv_wgmma_kernel: stage-1 deformable, stencil and corners staged in shared memory
+    Halo,       // conv_halo_kernel: stride 1, A fragments read with ldmatrix from a shared-memory input halo
+};
+
 // One 16-byte (8-channel) K slot: which tap of which source segment fills it.
 // plain conv: one entry per (chunk, slot).  RIC conv: one entry per (64-channel block, slot) - the
 // tap is the chunk's position inside the block.  Halo mode: per chunk as for a plain conv, plus one entry per
@@ -29,13 +44,6 @@ struct Slot {
     uint8_t pad_;
 };
 static_assert(sizeof(Slot) == 8, "Slot must be 8 bytes");
-
-// Host-side description of one K chunk (8 slots = 64 K elements) of the implicit GEMM; the kernel gets the masks as
-// launch constants (kmask_full / kmask_last).
-struct ChunkHdr {
-    uint8_t kmask;      // which of the 4 K=16 steps are issued against B tile 0
-    uint8_t kmask2;     // exact mode: which of A steps 0-1 (the hi half) are issued against B steps 2-3 (W_lo)
-};
 
 struct Seg {
     const __half* ptr;
@@ -75,12 +83,13 @@ struct ConvParams {
     int B, Hout, Wout;      // output geometry
     int Hin, Win;           // source buffer geometry (before the fused nearest x2)
     int Hv, Wv;             // virtual conv-input geometry = (Hin << up, Win << up)
-    int stride, up, ric, exact;
+    ConvMode mode;
+    int stride, up, exact;
     int nchunks, nblocks, Cout;
     int b_bytes;            // bytes per B stage = Cout x 128 (one chunk's weight tile in wpack)
-    // K-step masks (ChunkHdr semantics) as launch constants so the issuing warpgroups stay uniform:
-    // every chunk uses *_full except the ragged tail (tap mode: the last chunk; RIC: all chunks of the last
-    // channel block), which uses *_last
+    // K-step masks as launch constants so the issuing warpgroups stay uniform (kmask: which of the 4 K=16 steps are
+    // issued against B tile 0; kmask2, split fp16: which of A steps 0-1 are issued against B steps 2-3): every chunk uses
+    // *_full except the ragged tail (tap mode: the last chunk; RIC: all chunks of the last channel block), which uses *_last
     uint32_t kmask_full, kmask_last, kmask2_full, kmask2_last;
     const Slot* slots;      // plain: [nchunks][8]; RIC: [nblocks][8]
     const uint8_t* wpack;   // pre-swizzled B tiles
@@ -95,18 +104,15 @@ struct ConvParams {
     // source whose output pixel (oy, ox) of the Hout x Wout grid lands at (2*oy + sub_py, 2*ox + sub_px) of the
     // (2*Hout) x (2*Wout) output buffer
     int sub, sub_py, sub_px;
-    // halo mode (stride 1, no fused upsampling, not RIC): the channels are walked in blocks of 128 bytes per pixel; the
-    // (tile rows + ksize - 1) x (kTileW + ksize - 1) input halo of each block, origin (ty0 - pad_y, tx0 - pad_x), is staged in
-    // shared memory once and the A fragments of every tap are read from it straight into registers
-    int halo, ksize, pad_y, pad_x;
+    // halo mode: the channels are walked in blocks of 128 bytes per pixel; the (tile rows + ksize - 1) x (kTileW + ksize - 1)
+    // input halo of each block, origin (ty0 - pad_y, tx0 - pad_x), is staged in shared memory once and the A fragments of
+    // every tap are read from it straight into registers
+    int ksize, pad_y, pad_x;
     const Slot* hslots;     // [nblocks][8]: the channels of each 16-byte slot of a halo pixel
     int n128;               // Cout a multiple of 128: issue N = 128 wgmma instructions (else N = 64 / 32)
-    // RIC halo mode (ric = 1): the tile's stencil entries are staged in shared memory once per CTA and the input of each
-    // channel block (the tile +- 1 pixel in source coordinates) once per block; the corners of every tap are read from there
-    int ric_halo;
 };
 
 cudaError_t launch_conv(const ConvParams& p, cudaStream_t stream);
-size_t conv_smem_bytes(const ConvParams& p);
+size_t conv_smem_bytes(ConvMode mode, int cout, int ksize, int up);
 
 }  // namespace dsu

@@ -154,12 +154,11 @@ __device__ __forceinline__ void epilogue_batch(const ConvParams& p, const float*
 }
 
 // One accumulator row (= one output pixel, all Cout columns) per thread, read from the fp32 row `acc` the MMA
-// warpgroups staged in shared memory.  The `csplit` threads that share a row (chalf 0 .. csplit-1) split the 32-column
-// batches; the conv_12 tail needs a whole row in one thread, so only chalf 0 runs it.
-constexpr uint32_t kEpiAll = 0xFFFFu;   // variant mask (bit = variant index)
-template <uint32_t kMask = kEpiAll, bool kSub = false>
+// warpgroups staged in shared memory.  The two threads that share a row (chalf 0 / 1) split the 32-column batches; the
+// conv_12 tail needs a whole row in one thread, so only chalf 0 runs it.
+template <bool kSub>
 __device__ __forceinline__ void epilogue_row(const ConvParams& p, const float* s_par, const float* acc,
-                                             int n, int oy, int ox, int chalf, int csplit = 2) {
+                                             int n, int oy, int ox, int chalf) {
     const EpiParams& e = p.epi;
     const int C = p.Cout;
     const bool pix_ok = oy < p.Hout && ox < p.Wout;
@@ -168,7 +167,7 @@ __device__ __forceinline__ void epilogue_row(const ConvParams& p, const float* s
                              : (static_cast<size_t>(n) * p.Hout + oy) * p.Wout + ox;
     const int ncb = C / 32;
     const bool tail = e.w12 != nullptr;
-    const int cb_first = tail ? 0 : chalf, cb_step = tail ? 1 : csplit;
+    const int cb_first = tail ? 0 : chalf, cb_step = tail ? 1 : 2;
     const bool active = tail ? (chalf == 0) : (chalf < ncb);
     if (!active || !pix_ok) return;
     // uniform variant index: activation | second affine | lo plane
@@ -183,12 +182,9 @@ __device__ __forceinline__ void epilogue_row(const ConvParams& p, const float* s
             v[4 * c] = a.x; v[4 * c + 1] = a.y; v[4 * c + 2] = a.z; v[4 * c + 3] = a.w;
         }
         // variants the planner emits (engine.cu build_plan): act 0/1/2, second affine only with ReLU (conv_11_a.2), +8 = lo plane;
-        // kMask limits what a kernel instantiates (code size), anything else runs the cold run-time variant
-#define DSU_EPI_CASE(N, A, S2, LO)                                                                                        \
-    case N:                                                                                                               \
-        if constexpr ((kMask >> N) & 1u) { epilogue_batch<A, S2, LO>(p, s_par, v, opix, cb, tail, y3); handled = true; } \
-        break;
-        bool handled = false;
+        // anything else runs the cold run-time variant
+#define DSU_EPI_CASE(N, A, S2, LO) \
+    case N: epilogue_batch<A, S2, LO>(p, s_par, v, opix, cb, tail, y3); break;
         switch (variant) {
             DSU_EPI_CASE(0, 0, 0, false)
             DSU_EPI_CASE(1, 1, 0, false)
@@ -198,9 +194,8 @@ __device__ __forceinline__ void epilogue_row(const ConvParams& p, const float* s
             DSU_EPI_CASE(9, 1, 0, true)
             DSU_EPI_CASE(10, 2, 0, true)
             DSU_EPI_CASE(13, 1, 1, true)
-            default: break;
+            default: epilogue_batch<-1, -1, true>(p, s_par, v, opix, cb, tail, y3); break;
         }
-        if (!handled) epilogue_batch<-1, -1, true>(p, s_par, v, opix, cb, tail, y3);
 #undef DSU_EPI_CASE
     }
     if (tail) {

@@ -3,22 +3,20 @@
 // One CTA computes a tile of output pixels (GEMM M) of one frame for all Cout channels (GEMM N), K = taps x input
 // channels walked in 64-element chunks.  Two warpgroups (256 threads) do everything in turn.  Two mainloops:
 //
-// conv_wgmma_kernel (tap / RIC modes): a kTileH x kTileW patch (128 pixels).  Each chunk goes through a kStages-deep
+// conv_wgmma_kernel (Tap, Ric, RicHalo modes): a kTileH x kTileW patch (128 pixels).  Each chunk goes through a kStages-deep
 // ring of shared-memory stages holding the A operand (one 128-byte SWIZZLE_128B row per output pixel) and the chunk's
 // pre-swizzled weight tile (B operand, one 128-byte row per output channel).
 //   * PRODUCE chunk q + 2 while the MMAs of chunk q run.  Tap mode: each 16-byte slot of an A row is 8 channels of one
 //     tap of one concat segment (slot table), so stride 2 and fused nearest-x2 upsampling are pure address arithmetic
 //     (cp.async with zero fill at the border).  RIC (stage-1 deformable) layers blend the four bilinear corners of the
-//     rotated tap in registers and store the result; the corners come either straight from global memory (gather
-//     producer) or, in RIC halo mode, from the channel block's input halo (the tile +- 1 source pixel, staged once per
+//     rotated tap in registers and store the result; the corners come either straight from global memory (Ric, the gather
+//     producer) or, in RicHalo mode, from the channel block's input halo (the tile +- 1 source pixel, staged once per
 //     block with cp.async, double-buffered) with the tile's stencil staged once per CTA.  The weight tile is streamed
 //     with cp.async.
 //   * ISSUE wgmma: warpgroup w multiplies A rows 64w .. 64w+63 by the whole weight tile into its register accumulators.
 //
-// conv_halo_kernel (halo mode): the planner (engine.cu compile_layer) sends the first layer and every other stride-1 layer
-// without fused upsampling whose Cout <= 64 here, sub-pixel classes included.  A kRows x kTileW patch: kRows = 16 for
-// Cout <= 64; the first layer wider than 64 channels runs on 8-row tiles (register budget).  The concat is walked in channel blocks of
-// 128 bytes per pixel (8 groups of 8 channels, or 4 groups as hi + lo in exact mode).  The tile's input halo of a block
+// conv_halo_kernel (Halo mode): a halo_rows(Cout) x kTileW patch.  The concat is walked in channel blocks of 128 bytes per
+// pixel (8 groups of 8 channels, or 4 groups as hi + lo in exact mode).  The tile's input halo of a block
 // is loaded once with cp.async (double-buffered: block b + 1 lands while the taps of block b run) and every chunk's A
 // fragments are read from it with ldmatrix straight into registers (wgmma RS form, double-buffered across chunks), so
 // an input pixel crosses L2 once per block instead of once per tap.  Weight tiles stream through the same ring as above.
@@ -35,61 +33,43 @@ namespace dsu {
 
 namespace {
 
-// tap mode, RIC with the gather producer, RIC with the halo producer (fp16 / split fp16)
-constexpr int kModeTap = 0, kModeRic = 1, kModeRicExact = 2, kModeRicHalo = 3, kModeRicHaloExact = 4;
-
-struct SmemLayout {
-    uint32_t stage_bytes;   // A tile + B tile
-    uint32_t halo;          // RIC halo mode: two input halos of halo_bytes after the ring (halo_bytes = 0 otherwise)
-    uint32_t halo_bytes;
-    uint32_t sten;          // RIC halo mode: the tile's stencil entries, [rotated tap m][tile pixel] x 8 B
-    uint32_t par;           // epilogue parameters (the staged accumulators reuse the ring, halos and stencil)
-    uint32_t total;         // from the 1024-aligned base
-};
-
 __host__ __device__ inline uint32_t acc_pitch(int cout) { return static_cast<uint32_t>(cout) + 4; }   // floats per staged row
 
 __host__ __device__ inline uint32_t par_bytes(int cout) { return (7 * cout + 4) * 4; }
 
-// RIC halo mode: every corner of the 3 x 3 neighbourhoods of a tile lies in source rows (ty0 >> up) - 1 .. ((ty0 + kTileH) >> up)
+// RicHalo mode: every corner of the 3 x 3 neighbourhoods of a tile lies in source rows (ty0 >> up) - 1 .. ((ty0 + kTileH) >> up)
 // and columns (tx0 >> up) - 1 .. ((tx0 + kTileW) >> up): 10 x 18 pixels at up = 0, 6 x 10 with the fused nearest x2
 __host__ __device__ inline int ric_halo_rows(int up) { return (kTileH >> up) + 2; }
 __host__ __device__ inline int ric_halo_cols(int up) { return (kTileW >> up) + 2; }
 constexpr uint32_t kStenBytes = kTileM * 8 * 8;
 
-__host__ __device__ inline SmemLayout smem_layout(int cout, int b_bytes, bool ric_halo, int up) {
-    SmemLayout L;
-    L.stage_bytes = kABytes + b_bytes;
-    const uint32_t ring = kStages * L.stage_bytes, staged = kTileM * acc_pitch(cout) * 4;
-    L.halo = ring;
-    L.halo_bytes = ric_halo ? static_cast<uint32_t>(ric_halo_rows(up) * ric_halo_cols(up)) * 128u : 0u;
-    L.sten = L.halo + 2 * L.halo_bytes;
-    const uint32_t main_end = L.sten + (ric_halo ? kStenBytes : 0u);
-    L.par = ((main_end > staged ? main_end : staged) + 15u) & ~15u;
-    L.total = L.par + par_bytes(cout);
-    return L;
-}
-
-// halo mode: output rows per tile.  16 x 16 tiles halve the weight traffic per pixel; above 64 channels the two m64 blocks
+// Halo mode: output rows per tile.  16 x 16 tiles halve the weight traffic per pixel; above 64 channels the two m64 blocks
 // per warpgroup would not fit the register file next to the accumulators, so those layers keep 8 x 16.
-__host__ __device__ inline int halo_rows(int cout) { return cout <= 64 ? 16 : 8; }
+__host__ __device__ constexpr int halo_rows(int cout) { return cout <= 64 ? 16 : 8; }
 
-struct HaloLayout {
-    uint32_t stage_bytes;   // B tile of one chunk (ring of kStages at offset 0)
-    uint32_t halo;          // two halo buffers of halo_bytes
-    uint32_t halo_bytes;    // (rows + k - 1) x (kTileW + k - 1) pixels x 128 B
-    uint32_t zero;          // 16 zero bytes: the A rows of K-padding slots
-    uint32_t par;           // epilogue parameters (the staged accumulators reuse ring + halos)
+// Shared memory from the 1024-aligned base: a ring of kStages stages, then (RicHalo / Halo) two input-halo buffers and the
+// RicHalo stencil entries ([rotated tap m][tile pixel] x 8 B) or the Halo zero row (16 B, the A rows of K-padding slots), then
+// the epilogue parameters.  The staged fp32 accumulators reuse everything before `par`.
+struct SmemLayout {
+    uint32_t stage_bytes;   // A tile + B tile (Halo: B tile only, A lives in registers)
+    uint32_t halo;          // two input halos of halo_bytes each (halo_bytes = 0 in Tap / Ric mode)
+    uint32_t halo_bytes;
+    uint32_t aux;           // stencil (RicHalo) or zero row (Halo)
+    uint32_t par;
     uint32_t total;
 };
 
-__host__ __device__ inline HaloLayout halo_layout(int cout, int rows, int ksize) {
-    HaloLayout L;
-    L.stage_bytes = static_cast<uint32_t>(cout) * 128u;
+__host__ __device__ inline SmemLayout smem_layout(ConvMode mode, int cout, int ksize, int up) {
+    const bool halo = mode == ConvMode::Halo, ric_halo = mode == ConvMode::RicHalo;
+    const int rows = halo ? halo_rows(cout) : kTileH;
+    SmemLayout L;
+    L.stage_bytes = (halo ? 0u : static_cast<uint32_t>(kABytes)) + static_cast<uint32_t>(cout) * 128u;
     L.halo = kStages * L.stage_bytes;
-    L.halo_bytes = static_cast<uint32_t>((rows + ksize - 1) * (kTileW + ksize - 1)) * 128u;
-    L.zero = L.halo + 2 * L.halo_bytes;
-    const uint32_t main_end = L.zero + 16u, staged = static_cast<uint32_t>(rows * kTileW) * acc_pitch(cout) * 4u;
+    L.halo_bytes = halo       ? static_cast<uint32_t>((rows + ksize - 1) * (kTileW + ksize - 1)) * 128u
+                   : ric_halo ? static_cast<uint32_t>(ric_halo_rows(up) * ric_halo_cols(up)) * 128u : 0u;
+    L.aux = L.halo + 2 * L.halo_bytes;
+    const uint32_t main_end = L.aux + (halo ? 16u : ric_halo ? kStenBytes : 0u);
+    const uint32_t staged = static_cast<uint32_t>(rows * kTileW) * acc_pitch(cout) * 4u;
     L.par = ((main_end > staged ? main_end : staged) + 15u) & ~15u;
     L.total = L.par + par_bytes(cout);
     return L;
@@ -216,7 +196,7 @@ __device__ __forceinline__ void produce_ric(const ConvParams& p, int q, uint32_t
     }
 }
 
-// ---- RIC halo mode: what a CTA stages once, and the per-thread octants of its items (byte i = item row i)
+// ---- RicHalo mode: what a CTA stages once, and the per-thread octants of its items (byte i = item row i)
 struct RicTile {
     uint32_t halo, halo_bytes;  // two input-halo buffers: block b in buffer b & 1
     uint32_t sten;              // stencil entries [m][pixel], 8 B each
@@ -273,7 +253,7 @@ __device__ __forceinline__ void load_ric_halo(const ConvParams& p, int blk, uint
     }
 }
 
-// ---- RIC halo producer: the gather producer's items with the stencil entry from shared memory and the corners from the
+// ---- RicHalo producer: the gather producer's items with the stencil entry from shared memory and the corners from the
 // block's halo.  A corner (vy, vx) of the virtual image is halo pixel ((vy >> up) - y0, (vx >> up) - x0); rows and columns past
 // Hout / Wout in ragged tiles stay inside the halo and produce zeros (`live`).  Bank conflicts: a load phase of 8 threads is
 // one pixel's 8 slots (fp16), or 2 horizontally adjacent pixels x 4 groups (split fp16) whose corners of one sector are
@@ -319,15 +299,14 @@ __device__ __forceinline__ void produce_b(const ConvParams& p, int q, uint32_t d
     for (int i = tid; i < p.b_bytes / 16; i += kThreads) cp_async16(dst + 16u * i, src + 16 * i, 16u);
 }
 
-// chunk q: A rows and weight tile; in RIC halo mode the first chunk of block b also starts the halo of block b + 1
-template <int kMode>
+// chunk q: A rows and weight tile; in RicHalo mode the first chunk of block b also starts the halo of block b + 1
+template <ConvMode kMode, bool kExact>
 __device__ __forceinline__ void produce(const ConvParams& p, int q, uint32_t stage, int tid, int n, int ty0, int tx0, const RicTile& rt) {
-    if constexpr (kMode == kModeTap) {
+    if constexpr (kMode == ConvMode::Tap) {
         produce_tap(p, q, stage, tid, n, ty0, tx0);
-    } else if constexpr (kMode == kModeRic || kMode == kModeRicExact) {
-        produce_ric<kMode == kModeRicExact>(p, q, stage, tid, n, ty0, tx0);
+    } else if constexpr (kMode == ConvMode::Ric) {
+        produce_ric<kExact>(p, q, stage, tid, n, ty0, tx0);
     } else {
-        constexpr bool kExact = kMode == kModeRicHaloExact;
         const int blk = q / 9;
         if (q == 9 * blk && blk + 1 < p.nblocks)
             load_ric_halo<kExact>(p, blk + 1, rt.halo + static_cast<uint32_t>((blk + 1) & 1) * rt.halo_bytes, tid, n, ty0, tx0);
@@ -444,31 +423,31 @@ __device__ __forceinline__ void store_tile(const ConvParams& p, uint8_t* smem, c
     for (int i = 0; i < MB; ++i) {
         const int r = (tid & 127) + 128 * i;              // patch pixel; two threads per row split the 32-column batches
         const float* row = staged + r * acc_pitch(NC);
-        if (p.sub) epilogue_row<kEpiAll, true>(p, s_par, row, n, ty0 + (r >> 4), tx0 + (r & 15), tid >> 7);
-        else epilogue_row<kEpiAll, false>(p, s_par, row, n, ty0 + (r >> 4), tx0 + (r & 15), tid >> 7);
+        if (p.sub) epilogue_row<true>(p, s_par, row, n, ty0 + (r >> 4), tx0 + (r & 15), tid >> 7);
+        else epilogue_row<false>(p, s_par, row, n, ty0 + (r >> 4), tx0 + (r & 15), tid >> 7);
     }
 }
 
 }  // namespace
 
-// NC = Cout, PN = wgmma N per instruction (a divisor of NC: 32, 64 or 128)
+// NC = Cout, PN = wgmma N per instruction (a divisor of NC: 32, 64 or 128).  Tap mode reads the split-fp16 K steps from
+// the K masks, so it is instantiated with kExact = false for both precisions.
 //
-// RIC halo mode: the prologue stages the tile's stencil and the halo of channel block 0 (one cp.async group, waited for and
+// RicHalo mode: the prologue stages the tile's stencil and the halo of channel block 0 (one cp.async group, waited for and
 // made visible by a barrier before chunk 0 is produced).  Producers run two chunks ahead: chunk c is produced in iteration
 // c - 2 (chunks 0 and 1 in the prologue), so the first chunk of block b (c = 9b) is produced in iteration 9b - 2, and the
 // halo of block b + 1 is issued there, in that iteration's cp.async group.  Block b + 1 is first read by chunk 9b + 9, produced
 // in iteration 9b + 7, whose cp_async_wait<kStages - 3> (every group but the newest, i.e. up to iteration 9b + 5's) and
 // barrier make it visible.  It overwrites the buffer of block b - 1, whose last chunk 9b - 1 was produced in iteration 9b - 3,
 // before the barrier of iteration 9b - 2.
-template <int NC, int PN, int kMode>
+template <int NC, int PN, ConvMode kMode, bool kExact>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
-    constexpr bool kRicHalo = kMode == kModeRicHalo || kMode == kModeRicHaloExact;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_u32 = smem_u32(smem_raw);
     const uint32_t base = (raw_u32 + 1023u) & ~1023u;     // SWIZZLE_128B atoms are 1024-byte aligned
     uint8_t* smem = smem_raw + (base - raw_u32);
-    const SmemLayout L = smem_layout(NC, p.b_bytes, kRicHalo, p.up);
+    const SmemLayout L = smem_layout(kMode, NC, p.ksize, p.up);
     float* s_par = reinterpret_cast<float*>(smem + L.par);
 
     const int tid = threadIdx.x;
@@ -478,7 +457,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     const int tx0 = blockIdx.x * kTileW;
     const int nq = p.nchunks;
     // chunks with the ragged K tail: the last one (tap mode) or the 9 taps of the last channel block (RIC)
-    const int tail_from = kMode != kModeTap ? (p.nblocks - 1) * 9 : nq - 1;
+    const int tail_from = kMode != ConvMode::Tap ? (p.nblocks - 1) * 9 : nq - 1;
 
     load_epilogue_params(p, s_par, tid, kThreads);
 
@@ -486,9 +465,8 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
 #pragma unroll
     for (int i = 0; i < NC / 2; ++i) acc[0][i] = 0.0f;
 
-    RicTile rt{base + L.halo, L.halo_bytes, base + L.sten, 0u};
-    if constexpr (kRicHalo) {
-        constexpr bool kExact = kMode == kModeRicHaloExact;
+    RicTile rt{base + L.halo, L.halo_bytes, base + L.aux, 0u};
+    if constexpr (kMode == ConvMode::RicHalo) {
         rt.oct = load_ric_stencil<kExact>(p, rt.sten, tid, ty0, tx0);
         load_ric_halo<kExact>(p, 0, rt.halo, tid, n, ty0, tx0);
         cp_async_commit();
@@ -498,7 +476,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     // prologue: chunks 0 and 1; every iteration commits one cp.async group so that "chunk q has landed" is wait_group 1
 #pragma unroll
     for (int s = 0; s < kStages - 2; ++s) {
-        if (s < nq) produce<kMode>(p, s, base + s * L.stage_bytes, tid, n, ty0, tx0, rt);
+        if (s < nq) produce<kMode, kExact>(p, s, base + s * L.stage_bytes, tid, n, ty0, tx0, rt);
         cp_async_commit();
     }
     for (int q = 0; q < nq; ++q) {
@@ -512,7 +490,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
         mma_chunk<NC, PN>(acc[0], da, db, tail ? p.kmask_last : p.kmask_full, tail ? p.kmask2_last : p.kmask2_full);
         wgmma_commit();
         wgmma_wait<1>();                                  // this warpgroup's MMAs of chunk q - 1 have retired
-        if (q + kStages - 2 < nq) produce<kMode>(p, q + kStages - 2, base + ((q + kStages - 2) % kStages) * L.stage_bytes, tid, n, ty0, tx0, rt);
+        if (q + kStages - 2 < nq) produce<kMode, kExact>(p, q + kStages - 2, base + ((q + kStages - 2) % kStages) * L.stage_bytes, tid, n, ty0, tx0, rt);
         cp_async_commit();
     }
     wgmma_wait<0>();
@@ -527,17 +505,17 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
 // are free), ldmatrix the fragments of chunk q + 1, start the weight tile of chunk q + 2 and, in the first iteration of
 // block b, the halo of block b + 1 (it lands k^2 - 2 iterations before it is read; the buffer it overwrites was last
 // read in iteration b k^2 - 2).  The chunk loop is unrolled by two so that the fragment buffers have fixed registers.
-template <int NC, int PN, int kRows, bool kExact>
+template <int NC, int PN, bool kExact>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_halo_kernel(const __grid_constant__ ConvParams p) {
-    constexpr int kM = kRows * kTileW, MB = kM / 128;     // m64 blocks per warpgroup
+    constexpr int kRows = halo_rows(NC), kM = kRows * kTileW, MB = kM / 128;     // MB: m64 blocks per warpgroup
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_u32 = smem_u32(smem_raw);
     const uint32_t base = (raw_u32 + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base - raw_u32);
-    const HaloLayout L = halo_layout(NC, kRows, p.ksize);
+    const SmemLayout L = smem_layout(ConvMode::Halo, NC, p.ksize, 0);
     float* s_par = reinterpret_cast<float*>(smem + L.par);
-    const uint32_t zero = base + L.zero;
+    const uint32_t zero = base + L.aux;
 
     const int tid = threadIdx.x;
     const int wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
@@ -548,7 +526,7 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
     const int hw = kTileW + p.ksize - 1;
 
     load_epilogue_params(p, s_par, tid, kThreads);
-    if (tid < 4) reinterpret_cast<uint32_t*>(smem + L.zero)[tid] = 0u;
+    if (tid < 4) reinterpret_cast<uint32_t*>(smem + L.aux)[tid] = 0u;
 
     // halo pixel of this lane's A row in each m64 block, for the tap (0, 0) of the halo origin
     int pb[MB];
@@ -565,6 +543,7 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
     uint32_t a[2][MB][4][4];                              // [buffer][m64 block][K step][register]
 
     auto halo_buf = [&](int blk) { return base + L.halo + static_cast<uint32_t>(blk & 1) * L.halo_bytes; };
+
     // prologue: halo of block 0 + weights of chunk 0, then weights of chunk 1 (one cp.async group each)
     load_halo<kRows>(p, 0, halo_buf(0), tid, n, ty0, tx0);
     produce_b(p, 0, base, tid);
@@ -600,71 +579,45 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
     store_tile<NC, MB>(p, smem, s_par, acc, tid, n, ty0, tx0);
 }
 
-size_t conv_smem_bytes(const ConvParams& p) {
-    const uint32_t total = p.halo ? halo_layout(p.Cout, halo_rows(p.Cout), p.ksize).total
-                                  : smem_layout(p.Cout, p.b_bytes, p.ric && p.ric_halo, p.up).total;
-    return total + 1024;
-}
+size_t conv_smem_bytes(ConvMode mode, int cout, int ksize, int up) { return smem_layout(mode, cout, ksize, up).total + 1024; }
 
 namespace {
 
-// the attribute is per function and context: one flag per device
-template <typename K>
-cudaError_t allow_smem(K kernel, bool* attr_set) {
+template <ConvMode kMode, bool kExact, int NC, int PN>
+cudaError_t launch_one(const ConvParams& p, cudaStream_t stream) {
+    constexpr bool kHalo = kMode == ConvMode::Halo;
+    constexpr int kRows = kHalo ? halo_rows(NC) : kTileH;
+    void (*kernel)(ConvParams);
+    if constexpr (kHalo) kernel = conv_halo_kernel<NC, PN, kExact>;
+    else kernel = conv_wgmma_kernel<NC, PN, kMode, kExact>;
+    static bool attr_set[64] = {};                        // the attribute is per function and context: one flag per device
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    if (dev < 64 && attr_set[dev]) return cudaSuccess;
-    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess && dev < 64) attr_set[dev] = true;
-    return e;
-}
-
-template <int NC, int PN, int kMode>
-cudaError_t launch_nc(const ConvParams& p, cudaStream_t stream) {
-    static bool attr_set[64] = {};
-    cudaError_t e = allow_smem(conv_wgmma_kernel<NC, PN, kMode>, attr_set);
-    if (e != cudaSuccess) return e;
-    dim3 grid((p.Wout + kTileW - 1) / kTileW, (p.Hout + kTileH - 1) / kTileH, p.B);
-    conv_wgmma_kernel<NC, PN, kMode><<<grid, kThreads, conv_smem_bytes(p), stream>>>(p);
-    return cudaGetLastError();
-}
-
-template <int NC, int PN, bool kExact>
-cudaError_t launch_halo_nc(const ConvParams& p, cudaStream_t stream) {
-    constexpr int kRows = NC <= 64 ? 16 : 8;              // halo_rows(NC)
-    static bool attr_set[64] = {};
-    cudaError_t e = allow_smem(conv_halo_kernel<NC, PN, kRows, kExact>, attr_set);
+    if (e == cudaSuccess && !(dev < 64 && attr_set[dev])) {
+        e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        if (e == cudaSuccess && dev < 64) attr_set[dev] = true;
+    }
     if (e != cudaSuccess) return e;
     dim3 grid((p.Wout + kTileW - 1) / kTileW, (p.Hout + kRows - 1) / kRows, p.B);
-    conv_halo_kernel<NC, PN, kRows, kExact><<<grid, kThreads, conv_smem_bytes(p), stream>>>(p);
+    kernel<<<grid, kThreads, conv_smem_bytes(kMode, NC, p.ksize, p.up), stream>>>(p);
     return cudaGetLastError();
 }
 
-// halo mode in fp16 / split fp16 (numbered after the tap / RIC modes of launch_nc)
-constexpr int kModeHaloFp16 = 5, kModeHaloExact = 6;
-
-template <int kMode, int NC, int PN>
-cudaError_t launch_one(const ConvParams& p, cudaStream_t stream) {
-    if constexpr (kMode == kModeHaloFp16 || kMode == kModeHaloExact) return launch_halo_nc<NC, PN, kMode == kModeHaloExact>(p, stream);
-    else return launch_nc<NC, PN, kMode>(p, stream);
-}
-
-template <int kMode>
+template <ConvMode kMode, bool kExact>
 cudaError_t launch_mode(const ConvParams& p, cudaStream_t stream) {
     switch (p.Cout) {
-        case 32: return launch_one<kMode, 32, 32>(p, stream);
-        case 64: return launch_one<kMode, 64, 64>(p, stream);
-        case 96: return launch_one<kMode, 96, 32>(p, stream);
-        case 128: return p.n128 ? launch_one<kMode, 128, 128>(p, stream) : launch_one<kMode, 128, 64>(p, stream);
+        case 32: return launch_one<kMode, kExact, 32, 32>(p, stream);
+        case 64: return launch_one<kMode, kExact, 64, 64>(p, stream);
+        case 96: return launch_one<kMode, kExact, 96, 32>(p, stream);
+        case 128: return p.n128 ? launch_one<kMode, kExact, 128, 128>(p, stream) : launch_one<kMode, kExact, 128, 64>(p, stream);
         default: break;
     }
-    if constexpr (kMode != kModeRicExact && kMode != kModeRicHaloExact && kMode != kModeHaloExact) {              // split-fp16 configurations stop at 128 channels (engine.cu dsu_create)
+    if constexpr (!kExact) {              // split-fp16 configurations stop at 128 channels (engine.cu dsu_create)
         switch (p.Cout) {
-            case 160: return launch_one<kMode, 160, 32>(p, stream);
-            case 192: return launch_one<kMode, 192, 64>(p, stream);
-            case 224: return launch_one<kMode, 224, 32>(p, stream);
-            case 256: return p.n128 ? launch_one<kMode, 256, 128>(p, stream) : launch_one<kMode, 256, 64>(p, stream);
+            case 160: return launch_one<kMode, kExact, 160, 32>(p, stream);
+            case 192: return launch_one<kMode, kExact, 192, 64>(p, stream);
+            case 224: return launch_one<kMode, kExact, 224, 32>(p, stream);
+            case 256: return p.n128 ? launch_one<kMode, kExact, 256, 128>(p, stream) : launch_one<kMode, kExact, 256, 64>(p, stream);
             default: break;
         }
     }
@@ -674,15 +627,15 @@ cudaError_t launch_mode(const ConvParams& p, cudaStream_t stream) {
 }  // namespace
 
 cudaError_t launch_conv(const ConvParams& p, cudaStream_t stream) {
-    if (conv_smem_bytes(p) > 227 * 1024 || p.b_bytes != p.Cout * 128) return cudaErrorInvalidConfiguration;
-    if (p.halo) {
-        if (p.ric || p.stride != 1 || p.up || p.ksize < 2) return cudaErrorInvalidConfiguration;
-        return p.exact ? launch_mode<kModeHaloExact>(p, stream) : launch_mode<kModeHaloFp16>(p, stream);
+    if (conv_smem_bytes(p.mode, p.Cout, p.ksize, p.up) > 227 * 1024 || p.b_bytes != p.Cout * 128) return cudaErrorInvalidConfiguration;
+    switch (p.mode) {
+        case ConvMode::Tap: return launch_mode<ConvMode::Tap, false>(p, stream);
+        case ConvMode::Ric: return p.exact ? launch_mode<ConvMode::Ric, true>(p, stream) : launch_mode<ConvMode::Ric, false>(p, stream);
+        case ConvMode::RicHalo:
+            return p.exact ? launch_mode<ConvMode::RicHalo, true>(p, stream) : launch_mode<ConvMode::RicHalo, false>(p, stream);
+        case ConvMode::Halo: return p.exact ? launch_mode<ConvMode::Halo, true>(p, stream) : launch_mode<ConvMode::Halo, false>(p, stream);
     }
-    if (!p.ric) return p.ric_halo ? cudaErrorInvalidConfiguration : launch_mode<kModeTap>(p, stream);
-    if (p.stride != 1 || p.ksize != 3) return cudaErrorInvalidConfiguration;
-    if (p.ric_halo) return p.exact ? launch_mode<kModeRicHaloExact>(p, stream) : launch_mode<kModeRicHalo>(p, stream);
-    return p.exact ? launch_mode<kModeRicExact>(p, stream) : launch_mode<kModeRic>(p, stream);
+    return cudaErrorInvalidConfiguration;
 }
 
 }  // namespace dsu

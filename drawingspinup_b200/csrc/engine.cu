@@ -62,9 +62,10 @@ struct LayerDef {
     // wk = 3 is the kernel size of the stored weights; -1 = ordinary layer
     int sub = -1, wk = 0;
     int pad_y = 0, pad_x = 0;  // padding above / left of the window (compiled at finalize; a sub-pixel class pads (1 - py, 1 - px))
-    int first = 0;         // one <= 8-channel segment, stride 1, k > 3 (GeneratorJ.conv0): halo mode or tap mode (knob `first`)
     // compiled at finalize
-    int halo = 0;          // chunks in halo-mode order (channel block, tap, group); the kernel reads A from a shared-memory halo
+    int first = 0;         // conv0-shaped: one <= 8-channel segment, stride 1, k > 3
+    ConvMode mode = ConvMode::Tap;  // plan-time mode (Tap, Halo or Ric); conv_mode applies the run-time knobs
+    bool ric_halo_fits = false;     // the RicHalo shared-memory layout fits 227 KB
     int nchunks = 0, nblocks = 0;
     uint32_t kmask_full = 0xF, kmask_last = 0xF, kmask2_full = 0, kmask2_last = 0;
     Slot* d_slots = nullptr;
@@ -407,14 +408,15 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
             blocks.back().push_back(HSlot{0, 0, (int)si, s.choff + c8, s.wch0 + c8, std::max(0, std::min(8, s.wn - c8)), (int)blocks.back().size()});
         }
     }
+    L.first = (!L.ric && L.stride == 1 && L.up == 0 && L.sub < 0 && L.segs.size() == 1 && L.segs[0].nch <= 8 && k > 3 && L.pad == (k - 1) / 2) ? 1 : 0;
+    // Halo mode needs k >= 2: the halo of block b + 1 is loaded in the first chunk of block b and read k^2 - 1 chunks later
+    L.mode = L.ric ? ConvMode::Ric
+           : (L.stride == 1 && L.up == 0 && k >= 2 && (L.first || (E->knobs.halo && C <= 64))) ? ConvMode::Halo : ConvMode::Tap;
+    L.ric_halo_fits = L.ric && conv_smem_bytes(ConvMode::RicHalo, C, k, L.up) <= 227 * 1024;
+    L.nblocks = L.mode == ConvMode::Tap ? 0 : static_cast<int>(blocks.size());
     if (!L.ric) {
-        L.first = (L.stride == 1 && L.up == 0 && L.sub < 0 && L.segs.size() == 1 && L.segs[0].nch <= 8 && k > 3 && L.pad == (k - 1) / 2) ? 1 : 0;
-        // halo mode needs k >= 2: the halo of block b + 1 is loaded in the first chunk of block b and read k^2 - 1 chunks later.
-        // Only layers with Cout <= 64 (16 x 16 tiles) take it: on 8 x 16 tiles the 128-channel trunk and sub-pixel classes
-        // measured slower than tap mode (DESIGN section 7)
-        L.halo = (L.stride == 1 && L.up == 0 && k >= 2 && (L.first || (E->knobs.halo && C <= 64))) ? 1 : 0;
         std::vector<HSlot> all;
-        if (L.halo) {
+        if (L.mode == ConvMode::Halo) {
             // (block, tap, group): every full block is k^2 chunks of one tap each; the last block's groups are packed densely
             // over taps, so the chunk count equals tap mode's.  A one-group layer (conv0) gets the same chunks as in tap mode.
             for (const std::vector<HSlot>& blk : blocks) {
@@ -423,7 +425,6 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
                     for (int kw = 0; kw < k; ++kw)
                         for (HSlot h : blk) { h.kh = kh; h.kw = kw; all.push_back(h); }
             }
-            L.nblocks = static_cast<int>(blocks.size());
         } else {
             for (int kh = 0; kh < k; ++kh) {
                 for (int kw = 0; kw < k; ++kw)
@@ -433,7 +434,6 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
                             all.push_back(HSlot{kh, kw, (int)si, s.choff + c8, s.wch0 + c8, std::max(0, std::min(8, s.wn - c8)), 0});
                     }
             }
-            L.nblocks = 0;
         }
         for (size_t i = 0; i < all.size(); i += dpc) {
             std::vector<HSlot> ds(all.begin() + i, all.begin() + std::min(all.size(), i + dpc));
@@ -441,7 +441,6 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
             chunks.push_back(ds);
         }
     } else {
-        L.nblocks = static_cast<int>(blocks.size());
         for (const std::vector<HSlot>& blk : blocks) {
             push_dev_slots(blk, slots);                        // one slot row per BLOCK
             for (int tap = 0; tap < k * k; ++tap) {
@@ -452,7 +451,6 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
         }
     }
     L.nchunks = static_cast<int>(chunks.size());
-    std::vector<ChunkHdr> hdrs(L.nchunks);
     const size_t tile = static_cast<size_t>(C) * 128;
     std::vector<uint8_t> pack(static_cast<size_t>(L.nchunks) * tile, 0);
     size_t off = 0;
@@ -463,10 +461,6 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     for (int q = 0; q < L.nchunks; ++q) {
         const std::vector<HSlot>& ds = chunks[q];
         const int nd = static_cast<int>(ds.size());
-        const int steps = (nd + 1) / 2;                        // K=16 steps covering the data slots
-        ChunkHdr& hd = hdrs[q];
-        if (!exact) { hd.kmask = static_cast<uint8_t>((1 << steps) - 1); hd.kmask2 = 0; }
-        else { hd.kmask = static_cast<uint8_t>(((1 << steps) - 1) | (((1 << steps) - 1) << 2)); hd.kmask2 = static_cast<uint8_t>((1 << steps) - 1); }
         // B tile(s): row o = output channel, 128 B = 64 K elements, 16-byte slots XOR-swizzled by (row & 7)
         for (int o = 0; o < C; ++o)
             for (int d = 0; d < nd; ++d) {
@@ -481,8 +475,15 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
         off += tile;
     }
     pack.resize(off);
-    L.kmask_full = hdrs.front().kmask; L.kmask2_full = hdrs.front().kmask2;
-    L.kmask_last = hdrs.back().kmask; L.kmask2_last = hdrs.back().kmask2;
+    // K-step masks (ConvParams) of a chunk of nd data slots; only the ragged last chunk (tap / halo mode) or the chunks of
+    // the last channel block (RIC) have fewer data slots than the first chunk
+    auto kmasks = [&](size_t nd, uint32_t* km, uint32_t* km2) {
+        const uint32_t mask = (1u << ((nd + 1) / 2)) - 1;      // the K=16 steps covering the data slots
+        *km = exact ? mask | (mask << 2) : mask;
+        *km2 = exact ? mask : 0u;
+    };
+    kmasks(chunks.front().size(), &L.kmask_full, &L.kmask2_full);
+    kmasks(chunks.back().size(), &L.kmask_last, &L.kmask2_last);
     int rc_up;
     if ((rc_up = upload(&L.d_slots, slots))) return rc_up;
     if ((rc_up = upload(&L.d_hslots, hslots))) return rc_up;
@@ -665,17 +666,11 @@ int ensure_shape(dsu_engine* E, int B, int H, int W) {
     return DSU_OK;
 }
 
-// halo-mode plan, unless it is the first layer and knob `first` sends it to tap mode (same chunks in both orders)
-bool runs_halo(const dsu_engine* E, const LayerDef& L) { return L.halo && (!L.first || E->knobs.first != 0); }
-
-// RIC layer with the halo producer: knob `ric_halo` on and the layout (ring, two input halos, stencil, epilogue parameters)
-// fits 227 KB.  Every split-fp16 width (Cout <= 128) fits; in fp16, Cout >= 224 without fused upsampling (18-column halos)
-// does not and keeps the gather producer.  Same chunks and weight packing either way, so the knob may change at run time.
-bool runs_ric_halo(const dsu_engine* E, const LayerDef& L) {
-    if (!L.ric || !E->knobs.ric_halo) return false;
-    ConvParams p{};
-    p.Cout = L.cout; p.b_bytes = L.cout * 128; p.up = L.up; p.ric = 1; p.ric_halo = 1;
-    return conv_smem_bytes(p) <= 227 * 1024;
+// The mode a layer runs under the run-time knobs `first` and `ric_halo` (the rule: conv.cuh ConvMode)
+ConvMode conv_mode(const dsu_engine* E, const LayerDef& L) {
+    if (L.mode == ConvMode::Halo && L.first && !E->knobs.first) return ConvMode::Tap;
+    if (L.mode == ConvMode::Ric && L.ric_halo_fits && E->knobs.ric_halo) return ConvMode::RicHalo;
+    return L.mode;
 }
 
 int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgba, const uint8_t* alpha_src,
@@ -722,16 +717,14 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
         const int src_level = E->buf_level[L.segs[0].buf];
         p.Hin = H >> src_level; p.Win = W >> src_level;
         p.up = L.up; p.Hv = p.Hin << L.up; p.Wv = p.Win << L.up;
-        p.stride = L.stride; p.ric = L.ric; p.exact = E->exact ? 1 : 0;
+        p.mode = conv_mode(E, L); p.stride = L.stride; p.exact = E->exact ? 1 : 0;
         p.nchunks = L.nchunks; p.nblocks = L.nblocks; p.Cout = L.cout;
         p.b_bytes = L.cout * 128;
         p.kmask_full = L.kmask_full; p.kmask_last = L.kmask_last; p.kmask2_full = L.kmask2_full; p.kmask2_last = L.kmask2_last;
         if (L.sub >= 0) { p.sub = 1; p.sub_py = L.sub >> 1; p.sub_px = L.sub & 1; }
-        p.halo = runs_halo(E, L);
         p.ksize = L.k; p.pad_y = L.pad_y; p.pad_x = L.pad_x;
-        p.hslots = L.d_hslots;
         p.n128 = E->knobs.n128 != 0;
-        p.ric_halo = runs_ric_halo(E, L);
+        p.hslots = L.d_hslots;
         p.slots = L.d_slots; p.wpack = L.d_wpack;
         for (size_t i = 0; i < L.segs.size(); ++i) {
             p.seg[i].ptr = E->buf_hi[L.segs[i].buf];
@@ -1046,9 +1039,8 @@ const char* dsu_step_kernel(dsu_handle h, int32_t index) {
     if (!h || index < 0 || index >= static_cast<int>(h->steps.size())) return "";
     const Step& sp = h->steps[index];
     if (sp.type != 0) return sp.type == 1 ? "maxpool" : "instance_norm";
-    const LayerDef& L = h->layers[sp.layer];
-    if (L.ric) return runs_ric_halo(h, L) ? "ric_halo" : "ric";
-    return runs_halo(h, L) ? "halo" : "tap";
+    static const char* const kModeNames[] = {"tap", "ric", "ric_halo", "halo"};    // ConvMode order
+    return kModeNames[static_cast<int>(conv_mode(h, h->layers[sp.layer]))];
 }
 
 int dsu_frames_to_tensor(const uint8_t* color_dev, const uint8_t* pos_dev, const uint8_t* edge_dev,
