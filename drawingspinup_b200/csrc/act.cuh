@@ -1,0 +1,81 @@
+// Activation storage: how a value that crosses a kernel boundary sits in HBM (NHWC, DESIGN section 3), and the device
+// helpers that convert and store it.  A buffer holds one of three forms, chosen per handle by engine.cu act_out:
+//   * fp16, one plane (fp16 mode);
+//   * fp16 hi = fp16(v) and lo = fp16(v - hi), two planes (split-fp16 stage 2);
+//   * fp32 (split-fp16 stage 1: the RIC producers blend in fp32 and split after the blend).
+#pragma once
+#include <cuda_fp16.h>
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+namespace dsu {
+
+// Where a kernel stores channel c of pixel p: element p * pitch + choff + c of `f32` when it is non-null, else of `hi`
+// (and of `lo` when non-null).  All null: no store.
+struct ActOut {
+    __half* hi;
+    __half* lo;
+    float* f32;
+    int pitch, choff;
+};
+
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
+    __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<uint32_t*>(&h);
+}
+__device__ __forceinline__ float2 unpack_h2(uint32_t v) {
+    return __half22float2(*reinterpret_cast<const __half2*>(&v));
+}
+__device__ __forceinline__ void unpack8(const uint4& raw, float* f) {
+    float2 a = unpack_h2(raw.x), b = unpack_h2(raw.y), c = unpack_h2(raw.z), d = unpack_h2(raw.w);
+    f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
+}
+// 8 fp32 -> packed fp16 (hi plane only)
+__device__ __forceinline__ uint4 pack8(const float* f) {
+    return make_uint4(pack_h2(f[0], f[1]), pack_h2(f[2], f[3]), pack_h2(f[4], f[5]), pack_h2(f[6], f[7]));
+}
+// 8 fp32 -> packed fp16 hi and residual lo = fp16(v - hi)
+__device__ __forceinline__ void split8(const float* f, uint4& hi, uint4& lo) {
+    hi = pack8(f);
+    float r[8];
+    unpack8(hi, r);
+    lo.x = pack_h2(f[0] - r[0], f[1] - r[1]); lo.y = pack_h2(f[2] - r[2], f[3] - r[3]);
+    lo.z = pack_h2(f[4] - r[4], f[5] - r[5]); lo.w = pack_h2(f[6] - r[6], f[7] - r[7]);
+}
+
+// exact fp32 -> uint8 of custom_transforms.py:7-8: ((clip(x,-1,1)+1)/2*255) truncated, fp32 ops in order
+__device__ __forceinline__ uint8_t to_u8(float x) {
+    x = fminf(fmaxf(x, -1.0f), 1.0f);
+    float t = __fmul_rn(__fmul_rn(__fadd_rn(x, 1.0f), 0.5f), 255.0f);
+    return static_cast<uint8_t>(static_cast<int>(t));
+}
+
+// N (a multiple of 4) fp32 values -> fp32 at dst
+template <int N>
+__device__ __forceinline__ void store_f32(float* dst, const float* f) {
+#pragma unroll
+    for (int c = 0; c < N / 4; ++c) reinterpret_cast<float4*>(dst)[c] = make_float4(f[4 * c], f[4 * c + 1], f[4 * c + 2], f[4 * c + 3]);
+}
+
+// N (a multiple of 8) channels of pixel `pix`, starting at channel c of the view, in the view's form.  kLo = false: the
+// caller knows there is no lo plane, and the store does not test for one.
+template <int N, bool kLo = true>
+__device__ __forceinline__ void store_act(const ActOut& o, size_t pix, int c, const float* f) {
+    const size_t i = pix * o.pitch + o.choff + c;
+    if (o.f32) {
+        store_f32<N>(o.f32 + i, f);
+    } else if (o.hi) {
+        if (kLo && o.lo) {
+            uint4 h[N / 8], l[N / 8];
+#pragma unroll
+            for (int q = 0; q < N / 8; ++q) split8(f + 8 * q, h[q], l[q]);
+#pragma unroll
+            for (int q = 0; q < N / 8; ++q) { reinterpret_cast<uint4*>(o.hi + i)[q] = h[q]; reinterpret_cast<uint4*>(o.lo + i)[q] = l[q]; }
+        } else {
+#pragma unroll
+            for (int q = 0; q < N / 8; ++q) reinterpret_cast<uint4*>(o.hi + i)[q] = pack8(f + 8 * q);
+        }
+    }
+}
+
+}  // namespace dsu

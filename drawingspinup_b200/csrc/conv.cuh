@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "act.cuh"
+
 namespace dsu {
 
 constexpr int kTileH = 8;       // output patch rows per CTA
@@ -59,16 +61,9 @@ struct EpiParams {
     int act;                // 0 none, 1 ReLU, 2 LeakyReLU(0.2)
     int resid_in, resid_out;
     float* resid;           // fp32 residual stream [pix][Cout]
-    __half* out_hi;         // main fp16 output (after residual), optional ReLU
-    __half* out_lo;         // lo plane (exact mode) or null
-    int out_pitch, out_choff, out_relu;
-    __half* out2_hi;        // second, un-ReLU'd copy (skip connection) or null
-    __half* out2_lo;
-    int out2_pitch, out2_choff;
-    // stage 1 in split-fp16 mode keeps its activations in fp32 (same bytes as hi + lo planes; the RIC producers blend in fp32
-    // anyway and split after the blend): when non-null these replace out_hi/out_lo and out2_hi/out2_lo (same pitch / choff)
-    float* out_f32;
-    float* out2_f32;
+    ActOut out;             // main output (after residual), ReLU first when out_relu
+    ActOut out2;            // second, un-ReLU'd copy (skip connection)
+    int out_relu;
     // fused conv_12 (1x1, +bias, optional tanh) tail
     const float* w12;       // [3][Cout] or null
     const float* b12;       // [3]

@@ -1,37 +1,10 @@
-// Device helpers shared by the convolution kernels: fp16 pack/split, the exact uint8 conversion and
-// the fused epilogue (accumulator row -> BN/activation/residual -> fp16 NHWC / fp32 / uint8).
+// The fused epilogue of the convolution kernels: accumulator row -> BN/activation/residual -> activation stores
+// (act.cuh) / fp32 / uint8.
 #pragma once
 #include "conv.cuh"
 #include "ptx.cuh"
 
 namespace dsu {
-
-__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ float2 unpack_h2(uint32_t v) {
-    return __half22float2(*reinterpret_cast<const __half2*>(&v));
-}
-__device__ __forceinline__ void unpack8(const uint4& raw, float* f) {
-    float2 a = unpack_h2(raw.x), b = unpack_h2(raw.y), c = unpack_h2(raw.z), d = unpack_h2(raw.w);
-    f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
-}
-// 8 fp32 -> packed fp16 hi and residual lo = fp16(v - hi)
-__device__ __forceinline__ void split8(const float* f, uint4& hi, uint4& lo) {
-    hi.x = pack_h2(f[0], f[1]); hi.y = pack_h2(f[2], f[3]); hi.z = pack_h2(f[4], f[5]); hi.w = pack_h2(f[6], f[7]);
-    float r[8];
-    unpack8(hi, r);
-    lo.x = pack_h2(f[0] - r[0], f[1] - r[1]); lo.y = pack_h2(f[2] - r[2], f[3] - r[3]);
-    lo.z = pack_h2(f[4] - r[4], f[5] - r[5]); lo.w = pack_h2(f[6] - r[6], f[7] - r[7]);
-}
-
-// exact fp32 -> uint8 of custom_transforms.py:7-8: ((clip(x,-1,1)+1)/2*255) truncated, fp32 ops in order
-__device__ __forceinline__ uint8_t to_u8(float x) {
-    x = fminf(fmaxf(x, -1.0f), 1.0f);
-    float t = __fmul_rn(__fmul_rn(__fadd_rn(x, 1.0f), 0.5f), 255.0f);
-    return static_cast<uint8_t>(static_cast<int>(t));
-}
 
 // epilogue parameters in shared memory: [scale C][shift C][scale2 C][shift2 C][w12 3C][b12 4]
 __device__ __forceinline__ void load_epilogue_params(const ConvParams& p, float* s_par, int tid, int nthreads) {
@@ -50,34 +23,8 @@ __device__ __forceinline__ void load_epilogue_params(const ConvParams& p, float*
     if (p.epi.w12 && tid < 3) s_par[7 * C + tid] = p.epi.b12[tid];
 }
 
-// 8 fp32 -> packed fp16 (hi plane only)
-__device__ __forceinline__ uint4 pack8(const float* f) {
-    return make_uint4(pack_h2(f[0], f[1]), pack_h2(f[2], f[3]), pack_h2(f[4], f[5]), pack_h2(f[6], f[7]));
-}
-
-// 32 channels of one pixel -> fp16 NHWC (hi plane, plus the split-fp16 lo plane when kLo and `lo` is non-null)
-template <bool kLo>
-__device__ __forceinline__ void store32(__half* hi, __half* lo, const float* f) {
-    if (kLo && lo) {
-        uint4 h[4], l[4];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) split8(f + 8 * c, h[c], l[c]);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) { reinterpret_cast<uint4*>(hi)[c] = h[c]; reinterpret_cast<uint4*>(lo)[c] = l[c]; }
-    } else {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) reinterpret_cast<uint4*>(hi)[c] = pack8(f + 8 * c);
-    }
-}
-
-// 32 channels of one pixel -> fp32 NHWC (stage-1 activations of the split-fp16 mode)
-__device__ __forceinline__ void store32_f32(float* dst, const float* f) {
-#pragma unroll
-    for (int c = 0; c < 8; ++c) reinterpret_cast<float4*>(dst)[c] = make_float4(f[4 * c], f[4 * c + 1], f[4 * c + 2], f[4 * c + 3]);
-}
-
 // One 32-column batch of one accumulator row after the K-split partial sums were added: folded BN / bias, activation,
-// optional post-activation affine, residual stream, fp16 stores, conv_12 partial dot products.  The activation, the
+// optional post-activation affine, residual stream, activation stores, conv_12 partial dot products.  The activation, the
 // second affine and the lo plane are compile-time (dispatched once per row in epilogue_row), which keeps run-time tests
 // out of the 32-element loops.
 template <int kAct, int kScale2, bool kLo>   // kAct / kScale2 = -1: decided at run time (cold generic variant)
@@ -131,18 +78,12 @@ __device__ __forceinline__ void epilogue_batch(const ConvParams& p, const float*
 #pragma unroll
         for (int c = 0; c < 8; ++c) rp[c] = make_float4(f[4 * c], f[4 * c + 1], f[4 * c + 2], f[4 * c + 3]);
     }
-    if (e.out2_f32) store32_f32(e.out2_f32 + opix * e.out2_pitch + e.out2_choff + cb, f);
-    else if (e.out2_hi)
-        store32<kLo>(e.out2_hi + opix * e.out2_pitch + e.out2_choff + cb,
-                     e.out2_lo ? e.out2_lo + opix * e.out2_pitch + e.out2_choff + cb : nullptr, f);
+    store_act<32, kLo>(e.out2, opix, cb, f);
     if (e.out_relu) {
 #pragma unroll
         for (int c = 0; c < 32; ++c) f[c] = fmaxf(f[c], 0.0f);
     }
-    if (e.out_f32) store32_f32(e.out_f32 + opix * e.out_pitch + e.out_choff + cb, f);
-    else if (e.out_hi)
-        store32<kLo>(e.out_hi + opix * e.out_pitch + e.out_choff + cb,
-                     e.out_lo ? e.out_lo + opix * e.out_pitch + e.out_choff + cb : nullptr, f);
+    store_act<32, kLo>(e.out, opix, cb, f);
     if (tail) {
 #pragma unroll
         for (int c = 0; c < 32; ++c) {
@@ -171,7 +112,7 @@ __device__ __forceinline__ void epilogue_row(const ConvParams& p, const float* s
     const bool active = tail ? (chalf == 0) : (chalf < ncb);
     if (!active || !pix_ok) return;
     // uniform variant index: activation | second affine | lo plane
-    const int variant = e.act | (e.scale2 ? 4 : 0) | ((e.out_lo || e.out2_lo) ? 8 : 0);
+    const int variant = e.act | (e.scale2 ? 4 : 0) | ((e.out.lo || e.out2.lo) ? 8 : 0);
     float y3[3] = {0.0f, 0.0f, 0.0f};
     for (int cbi = cb_first; cbi < ncb; cbi += cb_step) {
         const int cb = cbi * 32;

@@ -5,7 +5,7 @@
 // BatchNorm (eval) is folded into per-channel scale/shift, conv weights are rounded to fp16
 // (hi [+lo]) and pre-swizzled into tensor-core tiles, skip connections / nearest-x2 upsampling /
 // stride / concat become slot tables, and the dead stage-1 smoother conv (models.py:348-350) is
-// dropped.  Activations live in NHWC fp16 workspace buffers owned by the handle.
+// dropped.  Activations live in NHWC workspace buffers owned by the handle, in one of the forms of act.cuh.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -156,7 +156,7 @@ struct dsu_engine {
     float* inorm_x = nullptr;      // norm_layer='instance_norm': raw fp32 output of the convolution being normalised
     float2* inorm_stats = nullptr; // [B][Cmax] (mean, 1/sqrt(var + eps))
     double* inorm_acc = nullptr;   // [B][Cmax][2] sum, sum of squares
-    size_t inorm_cap = 0, inorm_stats_cap = 0;
+    size_t inorm_cap = 0, inorm_stats_cap = 0;   // bytes of inorm_x, inorm_stats
     Level lv[3];
     std::map<std::pair<int, int>, std::vector<float>> user_offsets;
     uint8_t *io_color = nullptr, *io_pos = nullptr, *io_edge = nullptr, *io_out = nullptr;
@@ -607,55 +607,77 @@ int build_level(dsu_engine* E, Level& lv, int h, int w) {
 }
 
 // ------------------------------------------------------------------ workspace
+// Bytes of each workspace allocation at one shape: ensure_shape allocates them, dsu_workspace_bytes reports their sum
+struct Workspace {
+    size_t hi[NBUF], lo[NBUF];   // activation planes; f32_acts: one fp32 plane behind buf_hi, no lo plane
+    size_t resid, inorm_x, inorm_stats, inorm_acc;
+    size_t ric[3];               // the RIC stencil tables of each level (Level: lyx, oct, wh)
+    size_t total() const {
+        size_t t = resid + inorm_x + inorm_stats + inorm_acc;
+        for (int b = 0; b < NBUF; ++b) t += hi[b] + lo[b];
+        for (int l = 0; l < 3; ++l) t += ric[l];
+        return t;
+    }
+};
+
+Workspace workspace(const dsu_engine* E, int B, int H, int W) {
+    Workspace ws{};
+    for (int b = 0; b < NBUF; ++b) {
+        if (!E->buf_used[b]) continue;
+        const size_t n = static_cast<size_t>(B) * (H >> E->buf_level[b]) * (W >> E->buf_level[b]) * E->buf_C[b];
+        ws.hi[b] = n * (E->f32_acts ? sizeof(float) : sizeof(__half));
+        ws.lo[b] = E->exact && !E->f32_acts ? n * sizeof(__half) : 0;
+    }
+    if (E->cfg.resnet_blocks > 0) ws.resid = static_cast<size_t>(B) * (H >> 2) * (W >> 2) * E->cfg.filters[2] * sizeof(float);
+    int cmax = 0;
+    for (const LayerDef& L : E->layers)
+        if (L.inorm) {
+            ws.inorm_x = std::max(ws.inorm_x, static_cast<size_t>(B) * (H >> L.level_out) * (W >> L.level_out) * L.cout * sizeof(float));
+            cmax = std::max(cmax, L.cout);
+        }
+    ws.inorm_stats = static_cast<size_t>(B) * cmax * sizeof(float2);
+    ws.inorm_acc = static_cast<size_t>(B) * cmax * 2 * sizeof(double);
+    if (E->cfg.kind == DSU_KIND_GENERATORJ_RIC)
+        for (int l = 0; l < 3; ++l)
+            ws.ric[l] = static_cast<size_t>(H >> l) * (W >> l) * (8 * sizeof(float2) + sizeof(uint8_t) + 8 * sizeof(uint2));
+    return ws;
+}
+
 int ensure_shape(dsu_engine* E, int B, int H, int W) {
     if (B <= 0 || H <= 0 || W <= 0 || (H % 4) || (W % 4))
         return fail(DSU_E_INVALID, "frames must be [B>0, H, W] with H and W multiples of 4 (int(H/2), int(H/4) levels, models.py:296-300)");
+    const Workspace ws = workspace(E, B, H, W);
     for (int b = 0; b < NBUF; ++b) {
-        if (!E->buf_used[b]) continue;
-        const int l = E->buf_level[b];
-        // f32_acts: one fp32 plane (same bytes as the fp16 hi + lo planes) behind buf_hi, no lo plane
-        const size_t bytes = static_cast<size_t>(B) * (H >> l) * (W >> l) * E->buf_C[b] * (E->f32_acts ? sizeof(float) : sizeof(__half));
-        if (bytes > E->buf_cap[b]) {
-            if (E->buf_hi[b]) cudaFree(E->buf_hi[b]);
-            if (E->buf_lo[b]) cudaFree(E->buf_lo[b]);
-            E->buf_hi[b] = E->buf_lo[b] = nullptr;
-            CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->buf_hi[b]), bytes));
-            CUDA_TRY(cudaMemset(E->buf_hi[b], 0, bytes));
-            if (E->exact && !E->f32_acts) {
-                CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->buf_lo[b]), bytes));
-                CUDA_TRY(cudaMemset(E->buf_lo[b], 0, bytes));
-            }
-            E->buf_cap[b] = bytes;
+        if (ws.hi[b] <= E->buf_cap[b]) continue;
+        cudaFree(E->buf_hi[b]);
+        cudaFree(E->buf_lo[b]);
+        E->buf_hi[b] = E->buf_lo[b] = nullptr;
+        CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->buf_hi[b]), ws.hi[b]));
+        CUDA_TRY(cudaMemset(E->buf_hi[b], 0, ws.hi[b]));
+        if (ws.lo[b]) {
+            CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->buf_lo[b]), ws.lo[b]));
+            CUDA_TRY(cudaMemset(E->buf_lo[b], 0, ws.lo[b]));
         }
+        E->buf_cap[b] = ws.hi[b];
     }
-    const size_t rbytes = static_cast<size_t>(B) * (H >> 2) * (W >> 2) * E->cfg.filters[2] * sizeof(float);
-    if (E->cfg.resnet_blocks > 0 && rbytes > E->resid_cap) {
+    if (ws.resid > E->resid_cap) {
         if (E->resid) cudaFree(E->resid);
-        CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->resid), rbytes));
-        E->resid_cap = rbytes;
+        CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->resid), ws.resid));
+        E->resid_cap = ws.resid;
     }
-    if (E->cfg.norm == DSU_NORM_INSTANCE) {
-        size_t need = 0; int cmax = 0;
-        for (const LayerDef& L : E->layers)
-            if (L.inorm) {
-                need = std::max(need, static_cast<size_t>(B) * (H >> L.level_out) * (W >> L.level_out) * L.cout * sizeof(float));
-                cmax = std::max(cmax, L.cout);
-            }
-        if (need > E->inorm_cap) {
-            if (E->inorm_x) cudaFree(E->inorm_x);
-            E->inorm_x = nullptr;
-            CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->inorm_x), need));
-            E->inorm_cap = need;
-        }
-        const size_t sneed = static_cast<size_t>(B) * cmax;
-        if (sneed > E->inorm_stats_cap) {
-            if (E->inorm_stats) cudaFree(E->inorm_stats);
-            if (E->inorm_acc) cudaFree(E->inorm_acc);
-            E->inorm_stats = nullptr; E->inorm_acc = nullptr;
-            CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->inorm_stats), sneed * sizeof(float2)));
-            CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->inorm_acc), sneed * 2 * sizeof(double)));
-            E->inorm_stats_cap = sneed;
-        }
+    if (ws.inorm_x > E->inorm_cap) {
+        if (E->inorm_x) cudaFree(E->inorm_x);
+        E->inorm_x = nullptr;
+        CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->inorm_x), ws.inorm_x));
+        E->inorm_cap = ws.inorm_x;
+    }
+    if (ws.inorm_stats > E->inorm_stats_cap) {
+        if (E->inorm_stats) cudaFree(E->inorm_stats);
+        if (E->inorm_acc) cudaFree(E->inorm_acc);
+        E->inorm_stats = nullptr; E->inorm_acc = nullptr;
+        CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->inorm_stats), ws.inorm_stats));
+        CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->inorm_acc), ws.inorm_acc));
+        E->inorm_stats_cap = ws.inorm_stats;
     }
     if (E->cfg.kind == DSU_KIND_GENERATORJ_RIC)
         for (int l = 0; l < 3; ++l) {
@@ -664,6 +686,14 @@ int ensure_shape(dsu_engine* E, int B, int H, int W) {
         }
     E->B = B; E->H = H; E->W = W;
     return DSU_OK;
+}
+
+// The view of activation buffer `buf` from channel `choff` on, in the handle's storage form (act.cuh): where a kernel stores
+// (or max-pool reads).  buf < 0: no store.
+ActOut act_out(const dsu_engine* E, int buf, int choff) {
+    if (buf < 0) return ActOut{};
+    if (E->f32_acts) return ActOut{nullptr, nullptr, reinterpret_cast<float*>(E->buf_hi[buf]), E->buf_C[buf], choff};
+    return ActOut{E->buf_hi[buf], E->buf_lo[buf], nullptr, E->buf_C[buf], choff};
 }
 
 // The mode a layer runs under the run-time knobs `first` and `ric_halo` (the rule: conv.cuh ConvMode)
@@ -681,13 +711,7 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
         ++step_idx;
         if (sp.type == 1) {
             const int l = E->buf_level[sp.src];
-            if (E->f32_acts) {
-                CUDA_TRY(maxpool2_f32(reinterpret_cast<const float*>(E->buf_hi[sp.src]), E->buf_C[sp.src], sp.src_choff, B, H >> l, W >> l,
-                                      sp.C, reinterpret_cast<float*>(E->buf_hi[sp.dst]), E->buf_C[sp.dst], st));
-                continue;
-            }
-            CUDA_TRY(maxpool2(E->buf_hi[sp.src], E->buf_lo[sp.src], E->buf_C[sp.src], sp.src_choff, B, H >> l, W >> l, sp.C,
-                              E->buf_hi[sp.dst], E->buf_lo[sp.dst], E->buf_C[sp.dst], st));
+            CUDA_TRY(maxpool2(act_out(E, sp.src, sp.src_choff), act_out(E, sp.dst, 0), B, H >> l, W >> l, sp.C, st));
             continue;
         }
         const LayerDef& L = E->layers[sp.layer];
@@ -697,16 +721,7 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
             a.x = E->inorm_x; a.stats = E->inorm_stats;
             a.B = B; a.HW = (H >> L.level_out) * (W >> L.level_out); a.C = L.cout; a.act = L.act;
             a.resid = L.resid_out ? E->resid : nullptr;
-            if (L.out_buf >= 0) {
-                a.out_pitch = E->buf_C[L.out_buf]; a.out_choff = L.out_choff; a.out_relu = L.out_relu;
-                if (E->f32_acts) a.out_f32 = reinterpret_cast<float*>(E->buf_hi[L.out_buf]);
-                else { a.out_hi = E->buf_hi[L.out_buf]; a.out_lo = E->buf_lo[L.out_buf]; }
-            }
-            if (L.out2_buf >= 0) {
-                a.out2_pitch = E->buf_C[L.out2_buf]; a.out2_choff = 0;
-                if (E->f32_acts) a.out2_f32 = reinterpret_cast<float*>(E->buf_hi[L.out2_buf]);
-                else { a.out2_hi = E->buf_hi[L.out2_buf]; a.out2_lo = E->buf_lo[L.out2_buf]; }
-            }
+            a.out = act_out(E, L.out_buf, L.out_choff); a.out2 = act_out(E, L.out2_buf, 0); a.out_relu = L.out_relu;
             CUDA_TRY(instance_norm(a, E->inorm_acc, st));
             continue;
         }
@@ -726,30 +741,21 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
         p.n128 = E->knobs.n128 != 0;
         p.hslots = L.d_hslots;
         p.slots = L.d_slots; p.wpack = L.d_wpack;
-        for (size_t i = 0; i < L.segs.size(); ++i) {
-            p.seg[i].ptr = E->buf_hi[L.segs[i].buf];
-            p.seg[i].pitch = E->buf_C[L.segs[i].buf];
-            p.seg[i + kMaxSeg / 2].ptr = E->buf_lo[L.segs[i].buf];
-            p.seg[i + kMaxSeg / 2].pitch = E->buf_C[L.segs[i].buf];
+        for (size_t i = 0; i < L.segs.size(); ++i) {     // the producers read fp32 through the half-typed pointer (kEsz)
+            const ActOut a = act_out(E, L.segs[i].buf, 0);
+            p.seg[i].ptr = a.f32 ? reinterpret_cast<const __half*>(a.f32) : a.hi;
+            p.seg[i + kMaxSeg / 2].ptr = a.lo;
+            p.seg[i].pitch = p.seg[i + kMaxSeg / 2].pitch = a.pitch;
         }
         if (L.ric) { p.ric_lyx = E->lv[L.level_out].lyx; p.ric_oct = E->lv[L.level_out].oct; p.ric_wh = E->lv[L.level_out].wh; }
         EpiParams& e = p.epi;
         e.scale = L.d_scale; e.shift = L.d_shift; e.scale2 = L.d_scale2; e.shift2 = L.d_shift2;
         e.act = L.act; e.resid_in = L.resid_in; e.resid_out = L.resid_out; e.resid = E->resid;
-        if (L.out_buf >= 0) {
-            e.out_hi = E->buf_hi[L.out_buf]; e.out_lo = E->buf_lo[L.out_buf];
-            e.out_pitch = E->buf_C[L.out_buf]; e.out_choff = L.out_choff; e.out_relu = L.out_relu;
-            if (E->f32_acts) { e.out_f32 = reinterpret_cast<float*>(E->buf_hi[L.out_buf]); e.out_hi = nullptr; e.out_lo = nullptr; }
-        }
-        if (L.out2_buf >= 0) {
-            e.out2_hi = E->buf_hi[L.out2_buf]; e.out2_lo = E->buf_lo[L.out2_buf];
-            e.out2_pitch = E->buf_C[L.out2_buf]; e.out2_choff = 0;
-            if (E->f32_acts) { e.out2_f32 = reinterpret_cast<float*>(E->buf_hi[L.out2_buf]); e.out2_hi = nullptr; e.out2_lo = nullptr; }
-        }
+        e.out = act_out(E, L.out_buf, L.out_choff); e.out2 = act_out(E, L.out2_buf, 0); e.out_relu = L.out_relu;
         if (L.inorm) {
             // raw convolution output (+ bias) -> fp32 scratch through the residual-stream store; everything else happens in the type-2 step
             e.act = 0; e.resid_in = 0; e.resid_out = 1; e.resid = E->inorm_x; e.out_relu = 0;
-            e.out_hi = e.out_lo = e.out2_hi = e.out2_lo = nullptr; e.out_f32 = e.out2_f32 = nullptr;
+            e.out = e.out2 = ActOut{};
         }
         if (L.final) {
             e.w12 = E->d_w12; e.b12 = E->d_b12; e.tanh_flag = E->cfg.tanh;
@@ -899,8 +905,7 @@ int dsu_forward(dsu_handle h, const float* x_dev, int32_t B, int32_t H, int32_t 
     DEVICE_GUARD(h);
     if ((rc = ensure_shape(h, B, H, W))) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(ingest_f32(x_dev, B, h->cfg.input_channels, h->cin_pad, H, W, h->buf_hi[SK0], h->buf_lo[SK0],
-                        h->f32_acts ? reinterpret_cast<float*>(h->buf_hi[SK0]) : nullptr, h->buf_C[SK0], h->cfg.filters[0], st));
+    CUDA_TRY(ingest_f32(x_dev, B, h->cfg.input_channels, h->cin_pad, H, W, act_out(h, SK0, h->cfg.filters[0]), st));
     return run_network(h, B, H, W, y_dev, nullptr, nullptr, 0, st);
 }
 
@@ -914,8 +919,7 @@ int dsu_forward_u8(dsu_handle h, const uint8_t* color_dev, const uint8_t* pos_de
     DEVICE_GUARD(h);
     if ((rc = ensure_shape(h, B, H, W))) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(ingest_u8(color_dev, pos_dev, edge_dev, h->knobs.derive_edge, B, H, W, h->buf_hi[SK0], h->buf_lo[SK0],
-                       h->f32_acts ? reinterpret_cast<float*>(h->buf_hi[SK0]) : nullptr, h->buf_C[SK0], h->cfg.filters[0], st));
+    CUDA_TRY(ingest_u8(color_dev, pos_dev, edge_dev, h->knobs.derive_edge, B, H, W, act_out(h, SK0, h->cfg.filters[0]), st));
     return run_network(h, B, H, W, y_dev, out_rgba_dev, color_dev + 3, 4, st);
 }
 
@@ -947,21 +951,7 @@ int dsu_forward_u8_host(dsu_handle h, const uint8_t* color_host, const uint8_t* 
 }
 
 size_t dsu_workspace_bytes(dsu_handle h, int32_t B, int32_t H, int32_t W) {
-    if (!h) return 0;
-    size_t total = 0;
-    for (int b = 0; b < NBUF; ++b)
-        if (h->buf_used[b])
-            total += static_cast<size_t>(B) * (H >> h->buf_level[b]) * (W >> h->buf_level[b]) * h->buf_C[b] * 2 * (h->exact ? 2 : 1);
-    if (h->cfg.resnet_blocks > 0) total += static_cast<size_t>(B) * (H >> 2) * (W >> 2) * h->cfg.filters[2] * 4;
-    if (h->cfg.norm == DSU_NORM_INSTANCE) {
-        size_t need = 0;
-        for (const LayerDef& L : h->layers)
-            if (L.inorm) need = std::max(need, static_cast<size_t>(B) * (H >> L.level_out) * (W >> L.level_out) * L.cout * 4);
-        total += need;
-    }
-    if (h->cfg.kind == DSU_KIND_GENERATORJ_RIC)
-        for (int l = 0; l < 3; ++l) total += static_cast<size_t>(H >> l) * (W >> l) * 65;
-    return total;
+    return h ? workspace(h, B, H, W).total() : 0;
 }
 
 int dsu_forward_launches(dsu_handle h, int32_t B, int32_t H, int32_t W) {

@@ -1,5 +1,5 @@
-// HBM-bound per-pixel kernels around the convolution stack: frame ingest (uint8 / fp32 -> fp16 NHWC
-// hi[/lo] planes), 2x2 max-pool, and the stand-alone uint8 steps of the reference's frame loop
+// HBM-bound per-pixel kernels around the convolution stack: frame ingest (uint8 / fp32 -> activation
+// storage, act.cuh), 2x2 max-pool, and the stand-alone uint8 steps of the reference's frame loop
 // (custom_transforms.py:7-35, data.py:23-47, test_stage1.py:68-70, run_render.py:31-57).
 // One thread per pixel (or per 8-channel group), 128-bit accesses where the layout allows.
 #include "frames.cuh"
@@ -8,41 +8,12 @@ namespace dsu {
 
 namespace {
 
-__device__ __forceinline__ uint32_t pack_h2f(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
-
-// write 8 fp32 values as fp16 hi (and optional lo = fp16(v - hi)) 16-byte groups
-__device__ __forceinline__ void store8(__half* hi, __half* lo, const float* v) {
-    uint4 h;
-    h.x = pack_h2f(v[0], v[1]); h.y = pack_h2f(v[2], v[3]); h.z = pack_h2f(v[4], v[5]); h.w = pack_h2f(v[6], v[7]);
-    *reinterpret_cast<uint4*>(hi) = h;
-    if (lo) {
-        const __half2* hh = reinterpret_cast<const __half2*>(&h);
-        float r[8];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { float2 t = __half22float2(hh[i]); r[2 * i] = t.x; r[2 * i + 1] = t.y; }
-        uint4 l;
-        l.x = pack_h2f(v[0] - r[0], v[1] - r[1]); l.y = pack_h2f(v[2] - r[2], v[3] - r[3]);
-        l.z = pack_h2f(v[4] - r[4], v[5] - r[5]); l.w = pack_h2f(v[6] - r[6], v[7] - r[7]);
-        *reinterpret_cast<uint4*>(lo) = l;
-    }
-}
-
 // ToTensor + Normalize(0.5, 0.5) of custom_transforms.py:18-22: (u8/255 - 0.5)/0.5, fp32 ops in order
 __device__ __forceinline__ float norm_u8(uint8_t v) {
     return __fdiv_rn(__fsub_rn(__fdiv_rn(static_cast<float>(v), 255.0f), 0.5f), 0.5f);
 }
 
-// 8 fp32 values -> fp32 NHWC (stage 1 of the split-fp16 mode keeps fp32 activations)
-__device__ __forceinline__ void store8_f32(float* dst, const float* v) {
-    reinterpret_cast<float4*>(dst)[0] = make_float4(v[0], v[1], v[2], v[3]);
-    reinterpret_cast<float4*>(dst)[1] = make_float4(v[4], v[5], v[6], v[7]);
-}
-
-__global__ void ingest_f32_kernel(const float* __restrict__ x, int cin, int cpad, size_t npix_frame, size_t npix,
-                                  __half* hi, __half* lo, float* f32, int pitch, int choff) {
+__global__ void ingest_f32_kernel(const float* __restrict__ x, int cin, int cpad, size_t npix_frame, size_t npix, ActOut out) {
     const size_t p = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
     if (p >= npix) return;
     const size_t n = p / npix_frame, q = p % npix_frame;
@@ -51,8 +22,7 @@ __global__ void ingest_f32_kernel(const float* __restrict__ x, int cin, int cpad
         float v[8];
 #pragma unroll
         for (int c = 0; c < 8; ++c) v[c] = (g + c < cin) ? xp[static_cast<size_t>(g + c) * npix_frame] : 0.0f;
-        if (f32) store8_f32(f32 + p * pitch + choff + g, v);
-        else store8(hi + p * pitch + choff + g, lo ? lo + p * pitch + choff + g : nullptr, v);
+        store_act<8>(out, p, g, v);
     }
 }
 
@@ -72,11 +42,8 @@ __global__ void frames_to_tensor_kernel(const uchar4* __restrict__ color, const 
     if (mask_out) mask_out[p] = mask;
 }
 
-// 2x2 / stride 2 max-pool over NHWC fp16 (8 channels per thread).  With a lo plane the winner is
-// chosen on hi+lo and carries its own (hi, lo) pair.
-__global__ void maxpool2_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ in_lo, int in_pitch, int in_choff,
-                                int B, int Hin, int Win, int C,
-                                __half* out_hi, __half* out_lo, int out_pitch) {
+// 2x2 / stride 2 max-pool over NHWC fp16 (8 channels per thread)
+__global__ void maxpool2_kernel(const __half* __restrict__ in, int in_pitch, int B, int Hin, int Win, int C, __half* out, int out_pitch) {
     const int Ho = Hin / 2, Wo = Win / 2, G = C / 8;
     const size_t total = static_cast<size_t>(B) * Ho * Wo * G;
     const size_t t = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
@@ -86,36 +53,22 @@ __global__ void maxpool2_kernel(const __half* __restrict__ in_hi, const __half* 
     const int ox = static_cast<int>(op % Wo);
     const int oy = static_cast<int>((op / Wo) % Ho);
     const int n = static_cast<int>(op / (static_cast<size_t>(Wo) * Ho));
-    float best[8], bh[8], bl[8];
+    float best[8];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
         const size_t ip = (static_cast<size_t>(n) * Hin + 2 * oy + (k >> 1)) * Win + 2 * ox + (k & 1);
-        const uint4 rh = *reinterpret_cast<const uint4*>(in_hi + ip * in_pitch + in_choff + g * 8);
-        uint4 rl = make_uint4(0, 0, 0, 0);
-        if (in_lo) rl = *reinterpret_cast<const uint4*>(in_lo + ip * in_pitch + in_choff + g * 8);
-        const __half2* ph = reinterpret_cast<const __half2*>(&rh);
-        const __half2* pl = reinterpret_cast<const __half2*>(&rl);
+        float v[8];
+        unpack8(*reinterpret_cast<const uint4*>(in + ip * in_pitch + g * 8), v);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            const float2 h2 = __half22float2(ph[c]);
-            const float2 l2 = __half22float2(pl[c]);
-            const float v0 = h2.x + l2.x, v1 = h2.y + l2.y;
-            if (k == 0 || v0 > best[2 * c]) { best[2 * c] = v0; bh[2 * c] = h2.x; bl[2 * c] = l2.x; }
-            if (k == 0 || v1 > best[2 * c + 1]) { best[2 * c + 1] = v1; bh[2 * c + 1] = h2.y; bl[2 * c + 1] = l2.y; }
-        }
+        for (int c = 0; c < 8; ++c)      // strict > keeps the first maximum, like F.max_pool2d's value
+            if (k == 0 || v[c] > best[c]) best[c] = v[c];
     }
-    uint4 oh, ol;
-    oh.x = pack_h2f(bh[0], bh[1]); oh.y = pack_h2f(bh[2], bh[3]); oh.z = pack_h2f(bh[4], bh[5]); oh.w = pack_h2f(bh[6], bh[7]);
-    *reinterpret_cast<uint4*>(out_hi + op * out_pitch + g * 8) = oh;
-    if (out_lo) {
-        ol.x = pack_h2f(bl[0], bl[1]); ol.y = pack_h2f(bl[2], bl[3]); ol.z = pack_h2f(bl[4], bl[5]); ol.w = pack_h2f(bl[6], bl[7]);
-        *reinterpret_cast<uint4*>(out_lo + op * out_pitch + g * 8) = ol;
-    }
+    *reinterpret_cast<uint4*>(out + op * out_pitch + g * 8) = pack8(best);
 }
 
 // the same pool over fp32 NHWC (4 channels per thread)
-__global__ void maxpool2_f32_kernel(const float* __restrict__ in, int in_pitch, int in_choff, int B, int Hin, int Win, int C,
-                                    float* out, int out_pitch) {
+__global__ void maxpool2_f32_kernel(const float* __restrict__ in, int in_pitch, int B, int Hin, int Win, int C, float* out,
+                                    int out_pitch) {
     const int Ho = Hin / 2, Wo = Win / 2, G = C / 4;
     const size_t total = static_cast<size_t>(B) * Ho * Wo * G;
     const size_t t = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
@@ -129,7 +82,7 @@ __global__ void maxpool2_f32_kernel(const float* __restrict__ in, int in_pitch, 
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
         const size_t ip = (static_cast<size_t>(n) * Hin + 2 * oy + (k >> 1)) * Win + 2 * ox + (k & 1);
-        const float4 v = *reinterpret_cast<const float4*>(in + ip * in_pitch + in_choff + g * 4);
+        const float4 v = *reinterpret_cast<const float4*>(in + ip * in_pitch + g * 4);
         if (k == 0) best = v;
         else {      // strict > keeps the first maximum, like the fp16 kernel above and F.max_pool2d's value
             if (v.x > best.x) best.x = v.x;
@@ -141,15 +94,9 @@ __global__ void maxpool2_f32_kernel(const float* __restrict__ in, int in_pitch, 
     *reinterpret_cast<float4*>(out + op * out_pitch + g * 4) = best;
 }
 
-__device__ __forceinline__ uint8_t to_u8_dev(float x) {
-    x = fminf(fmaxf(x, -1.0f), 1.0f);
-    const float t = __fmul_rn(__fmul_rn(__fadd_rn(x, 1.0f), 0.5f), 255.0f);
-    return static_cast<uint8_t>(static_cast<int>(t));
-}
-
 __global__ void to_image_space_kernel(const float* __restrict__ x, uint8_t* __restrict__ out, size_t n) {
     const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
-    if (i < n) out[i] = to_u8_dev(x[i]);
+    if (i < n) out[i] = to_u8(x[i]);
 }
 
 __global__ void overlap_edge_kernel(const uint8_t* __restrict__ edge, uchar4* rgba, size_t npix) {
@@ -164,7 +111,7 @@ __global__ void compose_rgba_kernel(const float* __restrict__ y, const float* __
     const size_t n = p / npix_frame, r = p % npix_frame;
     const float* yp = y + n * 3 * npix_frame + r;
     const uint8_t a = static_cast<uint8_t>(static_cast<int>(__fmul_rn(mask[p], 255.0f)));   // (mask*255).astype(uint8)
-    out[p] = make_uchar4(to_u8_dev(yp[0]), to_u8_dev(yp[npix_frame]), to_u8_dev(yp[2 * npix_frame]), a);
+    out[p] = make_uchar4(to_u8(yp[0]), to_u8(yp[npix_frame]), to_u8(yp[2 * npix_frame]), a);
 }
 
 // pos2edge (run_render.py:31-57): per channel Sobel-3 (BORDER_REFLECT_101) in float64 on u8/255 with
@@ -204,8 +151,7 @@ __global__ void pos2edge_kernel(const uchar4* __restrict__ pos, int B, int H, in
 
 
 __global__ void ingest_u8_kernel(const uchar4* __restrict__ color, const uchar4* __restrict__ pos,
-                                 const uint8_t* __restrict__ edge, int derive_edge, int H, int W, size_t npix,
-                                 __half* hi, __half* lo, float* f32, int pitch, int choff) {
+                                 const uint8_t* __restrict__ edge, int derive_edge, int H, int W, size_t npix, ActOut out) {
     const size_t p = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
     if (p >= npix) return;
     uchar4 c = color[p];
@@ -221,8 +167,7 @@ __global__ void ingest_u8_kernel(const uchar4* __restrict__ color, const uchar4*
     }
     if (burn) { c.x = 0; c.y = 0; c.z = 0; }
     float v[8] = {norm_u8(c.x), norm_u8(c.y), norm_u8(c.z), mask, norm_u8(q.x), norm_u8(q.y), 0.0f, 0.0f};
-    if (f32) store8_f32(f32 + p * pitch + choff, v);
-    else store8(hi + p * pitch + choff, lo ? lo + p * pitch + choff : nullptr, v);
+    store_act<8>(out, p, 0, v);
 }
 
 
@@ -230,7 +175,7 @@ __global__ void ingest_u8_kernel(const uchar4* __restrict__ color, const uchar4*
 // biased variance) between a convolution and its activation.  The convolution's epilogue leaves its raw fp32 output
 // x[B][HW][C] in a scratch buffer; (1) per-(frame, channel) sum and sum of squares, accumulated in fp64 (slices of the
 // frame per block, one atomicAdd per (block, channel)); (2) mean / 1/sqrt(var + eps); (3) normalise, activation, and the
-// stores the fused epilogue would have done (residual stream, un-ReLU'd second copy, fp16 hi[/lo] or fp32 NHWC output).
+// stores the fused epilogue would have done (residual stream, un-ReLU'd second copy, output).
 __global__ void instnorm_stats_kernel(const float* __restrict__ x, int HW, int C, int rows_per_slice, double* acc) {
     __shared__ double s_sum[8][33], s_sq[8][33];
     const int lane = threadIdx.x & 31, row = threadIdx.x >> 5;              // 8 pixel rows x 32 channels per block step
@@ -282,34 +227,29 @@ __global__ void instnorm_apply_kernel(InstNormApply a) {
         if (a.act == 1) v[c] = fmaxf(v[c], 0.0f);
         else if (a.act == 2) v[c] = fmaxf(v[c], 0.2f * v[c]);
     }
-    if (a.resid) store8_f32(a.resid + pix * a.C + g * 8, v);
-    if (a.out2_f32) store8_f32(a.out2_f32 + pix * a.out2_pitch + a.out2_choff + g * 8, v);
-    else if (a.out2_hi) store8(a.out2_hi + pix * a.out2_pitch + a.out2_choff + g * 8,
-                               a.out2_lo ? a.out2_lo + pix * a.out2_pitch + a.out2_choff + g * 8 : nullptr, v);
+    if (a.resid) store_f32<8>(a.resid + pix * a.C + g * 8, v);
+    store_act<8>(a.out2, pix, g * 8, v);
     if (a.out_relu) {
 #pragma unroll
         for (int c = 0; c < 8; ++c) v[c] = fmaxf(v[c], 0.0f);
     }
-    if (a.out_f32) store8_f32(a.out_f32 + pix * a.out_pitch + a.out_choff + g * 8, v);
-    else if (a.out_hi) store8(a.out_hi + pix * a.out_pitch + a.out_choff + g * 8,
-                              a.out_lo ? a.out_lo + pix * a.out_pitch + a.out_choff + g * 8 : nullptr, v);
+    store_act<8>(a.out, pix, g * 8, v);
 }
 
 inline unsigned blocks_for(size_t n, int threads) { return static_cast<unsigned>((n + threads - 1) / threads); }
 
 }  // namespace
 
-cudaError_t ingest_f32(const float* x, int B, int cin, int cpad, int H, int W, __half* hi, __half* lo, float* f32, int pitch,
-                       int choff, cudaStream_t st) {
+cudaError_t ingest_f32(const float* x, int B, int cin, int cpad, int H, int W, const ActOut& out, cudaStream_t st) {
     const size_t npf = static_cast<size_t>(H) * W, np = npf * B;
-    ingest_f32_kernel<<<blocks_for(np, 256), 256, 0, st>>>(x, cin, cpad, npf, np, hi, lo, f32, pitch, choff);
+    ingest_f32_kernel<<<blocks_for(np, 256), 256, 0, st>>>(x, cin, cpad, npf, np, out);
     return cudaGetLastError();
 }
 cudaError_t ingest_u8(const uint8_t* color, const uint8_t* pos, const uint8_t* edge, int derive_edge, int B, int H, int W,
-                      __half* hi, __half* lo, float* f32, int pitch, int choff, cudaStream_t st) {
+                      const ActOut& out, cudaStream_t st) {
     const size_t np = static_cast<size_t>(H) * W * B;
     ingest_u8_kernel<<<blocks_for(np, 256), 256, 0, st>>>(reinterpret_cast<const uchar4*>(color), reinterpret_cast<const uchar4*>(pos), edge,
-                                                          derive_edge, H, W, np, hi, lo, f32, pitch, choff);
+                                                          derive_edge, H, W, np, out);
     return cudaGetLastError();
 }
 cudaError_t frames_to_tensor(const uint8_t* color, const uint8_t* pos, const uint8_t* edge, int B, int H, int W,
@@ -319,16 +259,15 @@ cudaError_t frames_to_tensor(const uint8_t* color, const uint8_t* pos, const uin
                                                                  reinterpret_cast<const uchar4*>(pos), edge, npf, np, pre, mask);
     return cudaGetLastError();
 }
-cudaError_t maxpool2(const __half* in_hi, const __half* in_lo, int in_pitch, int in_choff, int B, int Hin, int Win, int C,
-                     __half* out_hi, __half* out_lo, int out_pitch, cudaStream_t st) {
-    const size_t total = static_cast<size_t>(B) * (Hin / 2) * (Win / 2) * (C / 8);
-    maxpool2_kernel<<<blocks_for(total, 256), 256, 0, st>>>(in_hi, in_lo, in_pitch, in_choff, B, Hin, Win, C, out_hi, out_lo, out_pitch);
-    return cudaGetLastError();
-}
-cudaError_t maxpool2_f32(const float* in, int in_pitch, int in_choff, int B, int Hin, int Win, int C, float* out, int out_pitch,
-                         cudaStream_t st) {
-    const size_t total = static_cast<size_t>(B) * (Hin / 2) * (Win / 2) * (C / 4);
-    maxpool2_f32_kernel<<<blocks_for(total, 256), 256, 0, st>>>(in, in_pitch, in_choff, B, Hin, Win, C, out, out_pitch);
+cudaError_t maxpool2(const ActOut& in, const ActOut& out, int B, int Hin, int Win, int C, cudaStream_t st) {
+    if (in.lo || out.lo || !in.f32 != !out.f32) return cudaErrorInvalidValue;
+    const size_t opix = static_cast<size_t>(B) * (Hin / 2) * (Win / 2);
+    if (in.f32)
+        maxpool2_f32_kernel<<<blocks_for(opix * (C / 4), 256), 256, 0, st>>>(in.f32 + in.choff, in.pitch, B, Hin, Win, C,
+                                                                             out.f32 + out.choff, out.pitch);
+    else
+        maxpool2_kernel<<<blocks_for(opix * (C / 8), 256), 256, 0, st>>>(in.hi + in.choff, in.pitch, B, Hin, Win, C,
+                                                                         out.hi + out.choff, out.pitch);
     return cudaGetLastError();
 }
 cudaError_t to_image_space(const float* x, uint8_t* out, size_t n, cudaStream_t st) {

@@ -4,20 +4,19 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "act.cuh"
+
 namespace dsu {
 
-// `f32` non-null: write fp32 NHWC instead of the fp16 hi[/lo] planes (stage 1 of the split-fp16 mode)
-cudaError_t ingest_f32(const float* x, int B, int cin, int cpad, int H, int W, __half* hi, __half* lo, float* f32, int pitch,
-                       int choff, cudaStream_t st);
+cudaError_t ingest_f32(const float* x, int B, int cin, int cpad, int H, int W, const ActOut& out, cudaStream_t st);
 // edge == nullptr && derive_edge: burn the edges pos2edge would find in `pos` (run_render.py:31-57 fused into the ingest)
 cudaError_t ingest_u8(const uint8_t* color, const uint8_t* pos, const uint8_t* edge, int derive_edge, int B, int H, int W,
-                      __half* hi, __half* lo, float* f32, int pitch, int choff, cudaStream_t st);
-cudaError_t maxpool2_f32(const float* in, int in_pitch, int in_choff, int B, int Hin, int Win, int C, float* out, int out_pitch,
-                         cudaStream_t st);
+                      const ActOut& out, cudaStream_t st);
+// 2x2 / stride 2 max-pool of C channels from `in` to `out`, both fp16 or both fp32; a lo plane is an error (the split-fp16
+// mode pools only in stage 1, whose activations are fp32)
+cudaError_t maxpool2(const ActOut& in, const ActOut& out, int B, int Hin, int Win, int C, cudaStream_t st);
 cudaError_t frames_to_tensor(const uint8_t* color, const uint8_t* pos, const uint8_t* edge, int B, int H, int W,
                              float* pre, float* mask, cudaStream_t st);
-cudaError_t maxpool2(const __half* in_hi, const __half* in_lo, int in_pitch, int in_choff, int B, int Hin, int Win, int C,
-                     __half* out_hi, __half* out_lo, int out_pitch, cudaStream_t st);
 cudaError_t to_image_space(const float* x, uint8_t* out, size_t n, cudaStream_t st);
 cudaError_t overlap_edge(const uint8_t* edge, uint8_t* rgba, size_t npix, cudaStream_t st);
 cudaError_t compose_rgba(const float* y, const float* mask, int B, int H, int W, uint8_t* out, cudaStream_t st);
@@ -31,12 +30,9 @@ struct InstNormApply {
     int B, HW, C;
     int act;                 // 0 none, 1 ReLU, 2 LeakyReLU(0.2), applied after the normalisation
     float* resid;            // fp32 residual stream [pix][C] to write, or null
-    __half *out_hi, *out_lo; // main output (fp16 hi[/lo]) or out_f32; optional ReLU first
-    float* out_f32;
-    int out_pitch, out_choff, out_relu;
-    __half *out2_hi, *out2_lo;   // second copy taken before out_relu, or null
-    float* out2_f32;
-    int out2_pitch, out2_choff;
+    ActOut out;              // main output, ReLU first when out_relu
+    ActOut out2;             // second copy taken before out_relu
+    int out_relu;
 };
 cudaError_t instance_norm(const InstNormApply& a, double* acc /* [B][C][2] scratch */, cudaStream_t st);
 
