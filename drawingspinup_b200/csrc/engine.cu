@@ -155,7 +155,7 @@ struct dsu_engine {
     size_t resid_cap = 0;
     float* inorm_x = nullptr;      // norm_layer='instance_norm': raw fp32 output of the convolution being normalised
     float2* inorm_stats = nullptr; // [B][Cmax] (mean, 1/sqrt(var + eps))
-    double* inorm_acc = nullptr;   // [B][Cmax][2] sum, sum of squares
+    double* inorm_acc = nullptr;   // [B][Cmax][kInormMaxSlices][2] partial sum, sum of squares of each statistics slice
     size_t inorm_cap = 0, inorm_stats_cap = 0;   // bytes of inorm_x, inorm_stats
     Level lv[3];
     std::map<std::pair<int, int>, std::vector<float>> user_offsets;
@@ -636,7 +636,7 @@ Workspace workspace(const dsu_engine* E, int B, int H, int W) {
             cmax = std::max(cmax, L.cout);
         }
     ws.inorm_stats = static_cast<size_t>(B) * cmax * sizeof(float2);
-    ws.inorm_acc = static_cast<size_t>(B) * cmax * 2 * sizeof(double);
+    ws.inorm_acc = static_cast<size_t>(B) * cmax * kInormMaxSlices * 2 * sizeof(double);   // one slot per statistics slice
     if (E->cfg.kind == DSU_KIND_GENERATORJ_RIC)
         for (int l = 0; l < 3; ++l)
             ws.ric[l] = static_cast<size_t>(H >> l) * (W >> l) * (8 * sizeof(float2) + sizeof(uint8_t) + 8 * sizeof(uint2));

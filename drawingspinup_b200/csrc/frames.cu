@@ -173,9 +173,10 @@ __global__ void ingest_u8_kernel(const uchar4* __restrict__ color, const uchar4*
 
 // ---- nn.InstanceNorm2d (norm_layer='instance_norm', models.py:34-35; defaults: affine=False, no running stats, eps 1e-5,
 // biased variance) between a convolution and its activation.  The convolution's epilogue leaves its raw fp32 output
-// x[B][HW][C] in a scratch buffer; (1) per-(frame, channel) sum and sum of squares, accumulated in fp64 (slices of the
-// frame per block, one atomicAdd per (block, channel)); (2) mean / 1/sqrt(var + eps); (3) normalise, activation, and the
-// stores the fused epilogue would have done (residual stream, un-ReLU'd second copy, output).
+// x[B][HW][C] in a scratch buffer; (1) per-(frame, channel, slice) sum and sum of squares in fp64, each block storing its
+// partials to its own slot; (2) the slots summed in slice order, mean / 1/sqrt(var + eps); (3) normalise, activation, and
+// the stores the fused epilogue would have done (residual stream, un-ReLU'd second copy, output).  Every sum runs in one
+// fixed order, so the statistics are bit-reproducible run to run and independent of the batch a frame is in.
 __global__ void instnorm_stats_kernel(const float* __restrict__ x, int HW, int C, int rows_per_slice, double* acc) {
     __shared__ double s_sum[8][33], s_sq[8][33];
     const int lane = threadIdx.x & 31, row = threadIdx.x >> 5;              // 8 pixel rows x 32 channels per block step
@@ -194,16 +195,20 @@ __global__ void instnorm_stats_kernel(const float* __restrict__ x, int HW, int C
     if (row == 0 && c < C) {
 #pragma unroll
         for (int r = 1; r < 8; ++r) { s += s_sum[r][lane]; q += s_sq[r][lane]; }
-        atomicAdd(acc + (static_cast<size_t>(n) * C + c) * 2, s);
-        atomicAdd(acc + (static_cast<size_t>(n) * C + c) * 2 + 1, q);
+        double* slot = acc + ((static_cast<size_t>(n) * C + c) * kInormMaxSlices + blockIdx.y) * 2;
+        slot[0] = s;
+        slot[1] = q;
     }
 }
 
-__global__ void instnorm_finish_kernel(const double* __restrict__ acc, int total, int HW, float2* stats) {
+__global__ void instnorm_finish_kernel(const double* __restrict__ acc, int total, int HW, int slices, float2* stats) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
-    const double mean = acc[2 * i] / HW;
-    double var = acc[2 * i + 1] / HW - mean * mean;
+    const double* slot = acc + static_cast<size_t>(i) * kInormMaxSlices * 2;
+    double s = 0.0, q = 0.0;
+    for (int k = 0; k < slices; ++k) { s += slot[2 * k]; q += slot[2 * k + 1]; }
+    const double mean = s / HW;
+    double var = q / HW - mean * mean;
     var = var < 0.0 ? 0.0 : var;
     stats[i] = make_float2(static_cast<float>(mean), static_cast<float>(1.0 / sqrt(var + 1e-5)));
 }
@@ -291,13 +296,12 @@ cudaError_t pos2edge(const uint8_t* pos, int B, int H, int W, uint8_t* edge, cud
 
 cudaError_t instance_norm(const InstNormApply& a, double* acc, cudaStream_t st) {
     if (a.C % 8 || a.B < 1 || a.HW < 1 || !a.x || !a.stats || !acc) return cudaErrorInvalidValue;
-    cudaError_t e = cudaMemsetAsync(acc, 0, static_cast<size_t>(a.B) * a.C * 2 * sizeof(double), st);
-    if (e != cudaSuccess) return e;
     int slices = (a.HW + 4095) / 4096;                       // >= 4096 pixels per block and channel group, at most 64 slices
-    slices = slices > 64 ? 64 : slices;
+    slices = slices > kInormMaxSlices ? kInormMaxSlices : slices;
     const int rows = (a.HW + slices - 1) / slices;
     instnorm_stats_kernel<<<dim3((a.C + 31) / 32, slices, a.B), 256, 0, st>>>(a.x, a.HW, a.C, rows, acc);
-    instnorm_finish_kernel<<<blocks_for(static_cast<size_t>(a.B) * a.C, 128), 128, 0, st>>>(acc, a.B * a.C, a.HW, a.stats);
+    instnorm_finish_kernel<<<blocks_for(static_cast<size_t>(a.B) * a.C, 128), 128, 0, st>>>(acc, a.B * a.C, a.HW, slices,
+                                                                                          a.stats);
     const size_t total = static_cast<size_t>(a.B) * a.HW * (a.C / 8);
     instnorm_apply_kernel<<<blocks_for(total, 256), 256, 0, st>>>(a);
     return cudaGetLastError();

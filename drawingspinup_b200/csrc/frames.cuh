@@ -34,6 +34,9 @@ struct InstNormApply {
     ActOut out2;             // second copy taken before out_relu
     int out_relu;
 };
-cudaError_t instance_norm(const InstNormApply& a, double* acc /* [B][C][2] scratch */, cudaStream_t st);
+// Each plane's statistics are taken in min(64, ceil(HW / 4096)) slices of ceil(HW / slices) pixels, one block per (slice,
+// 32 channels, frame); `acc` holds one (sum, sum of squares) slot per slice, summed in slice order by the finish step.
+constexpr int kInormMaxSlices = 64;
+cudaError_t instance_norm(const InstNormApply& a, double* acc /* [B][C][kInormMaxSlices][2] scratch */, cudaStream_t st);
 
 }  // namespace dsu

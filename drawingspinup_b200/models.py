@@ -104,8 +104,9 @@ class _Generator(nn.Module):
         self.tanh = bool(tanh)
         self.filters = tuple(int(v) for v in filters)
         self.input_channels = int(input_channels)
-        # deterministic=True: bit-reproducible results run to run.  Every CTA accumulates its K chunks in a fixed order, so
-        # the engine is deterministic in both settings; the flag is kept for callers that request it explicitly.
+        # deterministic=True: bit-reproducible results run to run.  Every CTA accumulates its K chunks in a fixed order and
+        # the instance-norm statistics add their slices in slice order, so the engine is deterministic in both settings; the
+        # flag is kept for callers that request it explicitly.
         self.deterministic = bool(int(os.environ.get("DSU_DETERMINISTIC", "0"))) if deterministic is None else bool(deterministic)
         self.precision = precision or os.environ.get("DSU_PRECISION", "fp16x3")
         if self.precision not in capi.PRECISIONS:

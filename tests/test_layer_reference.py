@@ -188,8 +188,9 @@ def _ratio(got, ref, bound):
     return r.max().item(), r.pow(2).mean().sqrt().item(), r
 
 
-def _check_forward(tag, m, sd, stage, precision, args, x, y, knobs, halo, cache):
-    """Every launch of the plan against the reference of its layer (``halo``: DSU_HALO left on)."""
+def _check_forward(tag, m, sd, stage, precision, args, x, y, knobs, halo, cache, layers=None):
+    """Every launch of the plan against the reference of its layer (``halo``: DSU_HALO left on); ``layers``: only the
+    launches of these layers.  Returns ``{launch: (max, rms of err / bound)}``."""
     b, _, h, w = x.shape
     bufs = Buffers(m, stage, precision, args, b, h, w)
     cfg = _cfg(stage, args)
@@ -210,9 +211,11 @@ def _check_forward(tag, m, sd, stage, precision, args, x, y, knobs, halo, cache)
         assert torch.equal(bufs[P1], F.max_pool2d(bufs[O1], 2, 2))
     steps = [s for s in m.step_kernels() if s[1] not in ("maxpool", "instance_norm")]
     assert [_layer_of(n) for n, _ in steps if not n.endswith((".s1", ".s2", ".s3"))] == lr.layer_names(cfg)
-    done = {}
+    done, result = {}, {}
     for launch, mode in steps:
         layer = _layer_of(launch)
+        if layers is not None and layer not in layers:
+            continue
         cout = _cout(args, layer)
         # which mode each launch must run (the rule: conv.cuh ConvMode)
         if stage == 1:
@@ -255,6 +258,8 @@ def _check_forward(tag, m, sd, stage, precision, args, x, y, knobs, halo, cache)
               % (tag, "x".join(map(str, x.shape[:1] + x.shape[2:])), ",".join("%s=%d" % kv for kv in knobs.items()),
                  launch, mode, cout, pn, precision, worst, rms))
         assert worst <= 1.0, (tag, launch, mode, worst)
+        result[launch] = (worst, rms)
+    return result
 
 
 def _knob_settings(stage):

@@ -120,8 +120,9 @@ def _ric_conv(t, w, precision, h, wd, drop=(), rotate_octant=None):
     return acc.reshape(b, -1, h, wd)
 
 
-def emulate(sd, cfg, name, inputs, precision, out_form, resid=None, mut=()):
-    """A correct kernel of layer ``name`` (or one with the bug classes in ``mut``), float64 of what it stores."""
+def emulate(sd, cfg, name, inputs, precision, out_form, resid=None, mut=(), raw=False):
+    """A correct kernel of layer ``name`` (or one with the bug classes in ``mut``), float64 of what it stores.  ``raw``: the
+    fp32 convolution output (+ bias) the epilogue leaves for the instance-norm step instead."""
     s = lr.spec(cfg, name)
     w = sd[s["w"]].float()
     cout = w.shape[0]
@@ -182,6 +183,8 @@ def emulate(sd, cfg, name, inputs, precision, out_form, resid=None, mut=()):
     bias = sd.get(s["bias"]) if s["bias"] else None
     if bias is not None:
         acc = acc + bias.view(1, -1, 1, 1)
+    if raw:
+        return acc
     if s["norm"] and s["norm"] + ".weight" in sd:
         g, b_ = sd[s["norm"] + ".weight"], sd[s["norm"] + ".bias"]
         m, v = sd[s["norm"] + ".running_mean"], sd[s["norm"] + ".running_var"]
