@@ -34,13 +34,16 @@ __device__ __forceinline__ void unpack8(const uint4& raw, float* f) {
 __device__ __forceinline__ uint4 pack8(const float* f) {
     return make_uint4(pack_h2(f[0], f[1]), pack_h2(f[2], f[3]), pack_h2(f[4], f[5]), pack_h2(f[6], f[7]));
 }
-// 8 fp32 -> packed fp16 hi and residual lo = fp16(v - hi)
+// 2 fp32 -> packed fp16 hi and residual lo = fp16(v - hi)
+__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+    hi = pack_h2(a, b);
+    const float2 r = unpack_h2(hi);
+    lo = pack_h2(a - r.x, b - r.y);
+}
+// 8 fp32 -> packed fp16 hi and residual lo, two channels at a time
 __device__ __forceinline__ void split8(const float* f, uint4& hi, uint4& lo) {
-    hi = pack8(f);
-    float r[8];
-    unpack8(hi, r);
-    lo.x = pack_h2(f[0] - r[0], f[1] - r[1]); lo.y = pack_h2(f[2] - r[2], f[3] - r[3]);
-    lo.z = pack_h2(f[4] - r[4], f[5] - r[5]); lo.w = pack_h2(f[6] - r[6], f[7] - r[7]);
+    split2(f[0], f[1], hi.x, lo.x); split2(f[2], f[3], hi.y, lo.y);
+    split2(f[4], f[5], hi.z, lo.z); split2(f[6], f[7], hi.w, lo.w);
 }
 
 // exact fp32 -> uint8 of custom_transforms.py:7-8: ((clip(x,-1,1)+1)/2*255) truncated, fp32 ops in order

@@ -29,7 +29,9 @@ constexpr int kMaxSeg = 6;      // concat segments (second half = lo planes in e
 enum class ConvMode : int {
     Tap,        // conv_wgmma_kernel: each A slot gathered from global memory per (chunk, slot) with cp.async
     Ric,        // conv_wgmma_kernel: stage-1 deformable, the bilinear corners gathered from global memory
-    RicHalo,    // conv_wgmma_kernel: stage-1 deformable, stencil and corners staged in shared memory
+    RicHalo,    // stage-1 deformable, stencil and corners staged in shared memory: conv_halo_kernel blending the A fragments
+                // straight into registers for Cout <= 128 (every split-fp16 layer), conv_wgmma_kernel with a shared-memory
+                // A ring above (fp16 only)
     Halo,       // conv_halo_kernel: stride 1, A fragments read with ldmatrix from a shared-memory input halo
 };
 

@@ -3,9 +3,9 @@
 // One CTA computes a tile of output pixels (GEMM M) of one frame for all Cout channels (GEMM N), K = taps x input
 // channels walked in 64-element chunks.  Two warpgroups (256 threads) do everything in turn.  Two mainloops:
 //
-// conv_wgmma_kernel (Tap, Ric, RicHalo modes): a kTileH x kTileW patch (128 pixels).  Each chunk goes through a kStages-deep
-// ring of shared-memory stages holding the A operand (one 128-byte SWIZZLE_128B row per output pixel) and the chunk's
-// pre-swizzled weight tile (B operand, one 128-byte row per output channel).
+// conv_wgmma_kernel (Tap, Ric modes, and RicHalo for Cout > kRicRegMaxCout): a kTileH x kTileW patch (128 pixels).  Each
+// chunk goes through a kStages-deep ring of shared-memory stages holding the A operand (one 128-byte SWIZZLE_128B row per
+// output pixel) and the chunk's pre-swizzled weight tile (B operand, one 128-byte row per output channel).
 //   * PRODUCE chunk q + 2 while the MMAs of chunk q run.  Tap mode: each 16-byte slot of an A row is 8 channels of one
 //     tap of one concat segment (slot table), so stride 2 and fused nearest-x2 upsampling are pure address arithmetic
 //     (cp.async with zero fill at the border).  RIC (stage-1 deformable) layers blend the four bilinear corners of the
@@ -15,11 +15,13 @@
 //     with cp.async.
 //   * ISSUE wgmma: warpgroup w multiplies A rows 64w .. 64w+63 by the whole weight tile into its register accumulators.
 //
-// conv_halo_kernel (Halo mode): a halo_rows(Cout) x kTileW patch.  The concat is walked in channel blocks of 128 bytes per
-// pixel (8 groups of 8 channels, or 4 groups as hi + lo in exact mode).  The tile's input halo of a block
-// is loaded once with cp.async (double-buffered: block b + 1 lands while the taps of block b run) and every chunk's A
-// fragments are read from it with ldmatrix straight into registers (wgmma RS form, double-buffered across chunks), so
-// an input pixel crosses L2 once per block instead of once per tap.  Weight tiles stream through the same ring as above.
+// conv_halo_kernel (Halo mode, and RicHalo for Cout <= kRicRegMaxCout): the concat is walked in channel blocks of 128 bytes
+// per pixel (8 groups of 8 channels, or 4 groups as hi + lo in exact mode).  The tile's input halo of a block is loaded
+// once with cp.async (double-buffered: block b + 1 lands while the taps of block b run) and every chunk's A fragments are
+// built from it straight into registers (wgmma RS form, double-buffered across chunks), so an input pixel crosses L2 once
+// per block instead of once per tap, and no A tile passes through shared memory.  Halo mode (halo_rows(Cout) x kTileW
+// patch) reads the fragments with ldmatrix; RicHalo mode (8 x 16 patch) blends them from the rotated tap's corners in
+// the halo with the same helpers as the shared-memory RIC producers.  Weight tiles stream through the same ring as above.
 //
 // After the last chunk both kernels STAGE the accumulators to shared memory as fp32 rows and run the fused epilogue:
 // folded BN / activation / residual, fp16 NHWC (hi [+lo] planes), fp32 activations, the fp32 residual stream, or the
@@ -47,11 +49,32 @@ constexpr uint32_t kStenBytes = kTileM * 8 * 8;
 // per warpgroup would not fit the register file next to the accumulators, so those layers keep 8 x 16.
 __host__ __device__ constexpr int halo_rows(int cout) { return cout <= 64 ? 16 : 8; }
 
+// RicHalo mode: layers up to this width build their A fragments in registers (conv_halo_kernel); that covers every
+// split-fp16 layer (those configurations stop at 128 channels) and every layer of the default network.  Wider fp16 layers
+// keep the shared-memory A ring of conv_wgmma_kernel and its layout, so which of them fit the RicHalo layout at all
+// (engine.cu ric_halo_fits) is unchanged.  Compiled on the register path they would need 186-234 registers, without
+// spills, but they have not been measured there.
+constexpr int kRicRegMaxCout = 128;
+
+// whether a launch of this mode and width takes its A operand from registers (conv_halo_kernel)
+__host__ __device__ constexpr bool register_a(ConvMode mode, int cout) {
+    return mode == ConvMode::Halo || (mode == ConvMode::RicHalo && cout <= kRicRegMaxCout);
+}
+
+// CTAs per SM a conv_halo_kernel instantiation is built for.  A RicHalo CTA with A in registers spends most of each chunk
+// building the next chunk's fragments and at its barrier, with only two warps per SM sub-partition to hide the
+// shared-memory latency, so the tensor cores idle.  Up to 64 channels a second CTA fits: <= 128 registers per thread
+// (launch bounds; ptxas keeps two 8-byte values in a 16-byte stack slot) and <= 90 KB of shared memory each (ring
+// 4 x 8 KB, two 22.5 KB halos, 8 KB stencil, parameters).
+__host__ __device__ constexpr int ric_ctas_per_sm(ConvMode mode, int cout) {
+    return mode == ConvMode::RicHalo && cout <= 64 ? 2 : 1;
+}
+
 // Shared memory from the 1024-aligned base: a ring of kStages stages, then (RicHalo / Halo) two input-halo buffers and the
 // RicHalo stencil entries ([rotated tap m][tile pixel] x 8 B) or the Halo zero row (16 B, the A rows of K-padding slots), then
 // the epilogue parameters.  The staged fp32 accumulators reuse everything before `par`.
 struct SmemLayout {
-    uint32_t stage_bytes;   // A tile + B tile (Halo: B tile only, A lives in registers)
+    uint32_t stage_bytes;   // A tile + B tile (register A: B tile only)
     uint32_t halo;          // two input halos of halo_bytes each (halo_bytes = 0 in Tap / Ric mode)
     uint32_t halo_bytes;
     uint32_t aux;           // stencil (RicHalo) or zero row (Halo)
@@ -63,7 +86,7 @@ __host__ __device__ inline SmemLayout smem_layout(ConvMode mode, int cout, int k
     const bool halo = mode == ConvMode::Halo, ric_halo = mode == ConvMode::RicHalo;
     const int rows = halo ? halo_rows(cout) : kTileH;
     SmemLayout L;
-    L.stage_bytes = (halo ? 0u : static_cast<uint32_t>(kABytes)) + static_cast<uint32_t>(cout) * 128u;
+    L.stage_bytes = (register_a(mode, cout) ? 0u : static_cast<uint32_t>(kABytes)) + static_cast<uint32_t>(cout) * 128u;
     L.halo = kStages * L.stage_bytes;
     L.halo_bytes = halo       ? static_cast<uint32_t>((rows + ksize - 1) * (kTileW + ksize - 1)) * 128u
                    : ric_halo ? static_cast<uint32_t>(ric_halo_rows(up) * ric_halo_cols(up)) * 128u : 0u;
@@ -106,12 +129,35 @@ struct RicItems {
     static constexpr int kSlots = kExact ? 4 : 8, kRowsPer = kExact ? 2 : 4, kRowStep = kTileM / kRowsPer;
 };
 
-// torchvision's deform_conv2d bilinear rule with the engine's stencil tables: the centre tap copies corner (0, 0); a rotated
-// tap blends the 2x2 corner set of its sector with the stencil entry `entry()` (fp16: the four fp16 weights {w00,w01 | w10,w11};
-// split fp16: the fractions (ly, lx)), in the operation order of the reference port of the weights: w00*n00, then fma w01*n01,
-// w10*n10, w11*n11.  `fetch(cy, cx, h)` returns 16 source bytes of corner (cy, cx), zeros outside the (virtual, nearest-x2)
-// image: the 8 fp16 channels (h = 0), or fp32 channels 4h .. 4h + 3.  Both RIC producers go through here and differ only in
-// `entry` and `fetch`, so they write bit-identical A rows.
+// torchvision's deform_conv2d bilinear rule with the engine's stencil tables, per element: a rotated tap blends the 2x2
+// corner set of its sector in the operation order of the reference port of the weights: w00*n00, then fma w01*n01, w10*n10,
+// w11*n11.  fp16: the stencil entry holds the four fp16 weights {w00,w01 | w10,w11} and one call blends a packed-half2 word
+// (two channels).  Split fp16: the entry holds the fractions (ly, lx), the weights and the blend are fp32 with explicit
+// rounding, one channel per call.  Every RIC A producer goes through these two functions, so they all agree bit for bit.
+struct RicWeightsH { __half2 w00, w01, w10, w11; };
+struct RicWeightsF { float w0, w1, w2, w3; };
+
+__device__ __forceinline__ __half2 h2_of(uint32_t v) { return *reinterpret_cast<const __half2*>(&v); }
+
+__device__ __forceinline__ RicWeightsH ric_weights(uint2 wv) {
+    const __half2 wa = h2_of(wv.x), wb = h2_of(wv.y);
+    return {__low2half2(wa), __high2half2(wa), __low2half2(wb), __high2half2(wb)};
+}
+__device__ __forceinline__ RicWeightsF ric_weights(float2 l) {
+    const float hy = 1.0f - l.x, hx = 1.0f - l.y;
+    return {__fmul_rn(hy, hx), __fmul_rn(hy, l.y), __fmul_rn(l.x, hx), __fmul_rn(l.x, l.y)};
+}
+__device__ __forceinline__ uint32_t ric_blend(const RicWeightsH& w, uint32_t n00, uint32_t n01, uint32_t n10, uint32_t n11) {
+    const __half2 o = __hfma2(w.w11, h2_of(n11), __hfma2(w.w10, h2_of(n10), __hfma2(w.w01, h2_of(n01), __hmul2(w.w00, h2_of(n00)))));
+    return *reinterpret_cast<const uint32_t*>(&o);
+}
+__device__ __forceinline__ float ric_blend(const RicWeightsF& w, float v00, float v01, float v10, float v11) {
+    return __fmaf_rn(w.w3, v11, __fmaf_rn(w.w2, v10, __fmaf_rn(w.w1, v01, __fmul_rn(w.w0, v00))));
+}
+
+// One A-row item of the shared-memory-A producers: the centre tap copies corner (0, 0); a rotated tap blends its corners
+// with the stencil entry `entry()`.  `fetch(cy, cx, h)` returns 16 source bytes of corner (cy, cx), zeros outside the
+// (virtual, nearest-x2) image: the 8 fp16 channels (h = 0), or fp32 channels 4h .. 4h + 3.
 template <bool kExact, typename Entry, typename Fetch>
 __device__ __forceinline__ void ric_item(bool centre, const Entry& entry, const Fetch& fetch, uint32_t row, int d, uint32_t swz) {
     if constexpr (!kExact) {
@@ -119,17 +165,10 @@ __device__ __forceinline__ void ric_item(bool centre, const Entry& entry, const 
         if (centre) {
             out = fetch(0, 0, 0);
         } else {
-            const uint2 wv = entry();
-            const __half2 wa = *reinterpret_cast<const __half2*>(&wv.x), wb = *reinterpret_cast<const __half2*>(&wv.y);
-            const __half2 w00 = __low2half2(wa), w01 = __high2half2(wa), w10 = __low2half2(wb), w11 = __high2half2(wb);
+            const RicWeightsH w = ric_weights(entry());
             const uint4 n00 = fetch(0, 0, 0), n01 = fetch(0, 1, 0), n10 = fetch(1, 0, 0), n11 = fetch(1, 1, 0);
-            const __half2* h00 = reinterpret_cast<const __half2*>(&n00);
-            const __half2* h01 = reinterpret_cast<const __half2*>(&n01);
-            const __half2* h10 = reinterpret_cast<const __half2*>(&n10);
-            const __half2* h11 = reinterpret_cast<const __half2*>(&n11);
-            __half2* o = reinterpret_cast<__half2*>(&out);
-#pragma unroll
-            for (int c = 0; c < 4; ++c) o[c] = __hfma2(w11, h11[c], __hfma2(w10, h10[c], __hfma2(w01, h01[c], __hmul2(w00, h00[c]))));
+            out = make_uint4(ric_blend(w, n00.x, n01.x, n10.x, n11.x), ric_blend(w, n00.y, n01.y, n10.y, n11.y),
+                             ric_blend(w, n00.z, n01.z, n10.z, n11.z), ric_blend(w, n00.w, n01.w, n10.w, n11.w));
         }
         st_shared_v4(row + ((static_cast<uint32_t>(d) ^ swz) << 4), out);
     } else {
@@ -143,13 +182,11 @@ __device__ __forceinline__ void ric_item(bool centre, const Entry& entry, const 
         if (centre) {
             load8(0, 0, f);
         } else {
-            const float2 l = entry();
-            const float hy = 1.0f - l.x, hx = 1.0f - l.y;
-            const float w0 = __fmul_rn(hy, hx), w1 = __fmul_rn(hy, l.y), w2 = __fmul_rn(l.x, hx), w3 = __fmul_rn(l.x, l.y);
+            const RicWeightsF w = ric_weights(entry());
             float v00[8], v01[8], v10[8], v11[8];
             load8(0, 0, v00); load8(0, 1, v01); load8(1, 0, v10); load8(1, 1, v11);
 #pragma unroll
-            for (int c = 0; c < 8; ++c) f[c] = __fmaf_rn(w3, v11[c], __fmaf_rn(w2, v10[c], __fmaf_rn(w1, v01[c], __fmul_rn(w0, v00[c]))));
+            for (int c = 0; c < 8; ++c) f[c] = ric_blend(w, v00[c], v01[c], v10[c], v11[c]);
         }
         uint4 hi, lo;
         split8(f, hi, lo);
@@ -208,8 +245,7 @@ struct RicTile {
 // Hout x Wout.  The octants go to registers: an item's output pixel never changes across chunks.  (They are read with
 // plain loads: a tile row of octant bytes is not 4-byte aligned when Wout is not a multiple of 4.)
 template <bool kExact>
-__device__ __forceinline__ uint32_t load_ric_stencil(const ConvParams& p, uint32_t sten, int tid, int ty0, int tx0) {
-    using It = RicItems<kExact>;
+__device__ __forceinline__ void stage_ric_stencil(const ConvParams& p, uint32_t sten, int tid, int ty0, int tx0) {
     const uint8_t* table = kExact ? reinterpret_cast<const uint8_t*>(p.ric_lyx) : reinterpret_cast<const uint8_t*>(p.ric_wh);
     for (int i = tid; i < kTileM * 8; i += kThreads) {
         const int r = i >> 3, m = i & 7;
@@ -218,13 +254,21 @@ __device__ __forceinline__ uint32_t load_ric_stencil(const ConvParams& p, uint32
         const size_t e = ok ? static_cast<size_t>(oy) * p.Wout + ox : 0;
         cp_async8(sten + static_cast<uint32_t>(m * kTileM + r) * 8u, table + (e * 8 + m) * 8, ok ? 8u : 0u);
     }
+}
+
+// the octant of tile pixel r (0 outside Hout x Wout)
+__device__ __forceinline__ uint32_t ric_oct(const ConvParams& p, int r, int ty0, int tx0) {
+    const int oy = ty0 + (r >> 4), ox = tx0 + (r & 15);
+    return (oy < p.Hout && ox < p.Wout) ? static_cast<uint32_t>(__ldg(p.ric_oct + static_cast<size_t>(oy) * p.Wout + ox)) : 0u;
+}
+
+template <bool kExact>
+__device__ __forceinline__ uint32_t load_ric_stencil(const ConvParams& p, uint32_t sten, int tid, int ty0, int tx0) {
+    using It = RicItems<kExact>;
+    stage_ric_stencil<kExact>(p, sten, tid, ty0, tx0);
     uint32_t oct = 0;
 #pragma unroll
-    for (int i = 0; i < It::kRowsPer; ++i) {
-        const int r = tid / It::kSlots + It::kRowStep * i;
-        const int oy = ty0 + (r >> 4), ox = tx0 + (r & 15);
-        if (oy < p.Hout && ox < p.Wout) oct |= static_cast<uint32_t>(__ldg(p.ric_oct + static_cast<size_t>(oy) * p.Wout + ox)) << (8 * i);
-    }
+    for (int i = 0; i < It::kRowsPer; ++i) oct |= ric_oct(p, tid / It::kSlots + It::kRowStep * i, ty0, tx0) << (8 * i);
     return oct;
 }
 
@@ -290,6 +334,129 @@ __device__ __forceinline__ void produce_ric_halo(const ConvParams& p, int q, uin
             else return raw;
         };
         ric_item<kExact>(t == 4, entry, fetch, a + static_cast<uint32_t>(r) * 128u, d, static_cast<uint32_t>(r & 7));
+    }
+}
+
+// ---- RicHalo mode with A in registers (Cout <= kRicRegMaxCout).  Lane l of warp w in warpgroup wg holds the A fragments
+// of tile pixels r = 64 wg + 16 w + l / 4 and r + 8 (fragment rows l / 4 and l / 4 + 8: tile row 4 wg + w, columns l / 4 and
+// l / 4 + 8), columns 2 (l % 4), +1 of the 16-byte slots 2k and 2k + 1 of K step k: the layout ldsm_x4 returns and mma_rs
+// takes, a[k][0 | 1] = slot 2k of pixel r | r + 8, a[k][2 | 3] = slot 2k + 1.  What a lane needs in every chunk:
+struct RicLane {
+    int r;              // tile pixel of fragment row l / 4 (the other row is r + 8)
+    int oy, ox;         // its output pixel (the other one is (oy, ox + 8))
+    uint32_t live;      // bit j: pixel r + 8j lies inside Hout x Wout
+    uint32_t oct;       // byte j: octant of pixel r + 8j; byte 2 (fp16): octant of the ldmatrix row pixel
+    int ax;             // fp16: output column of the pixel whose row address this lane gives ldmatrix (row oy, slot 2k + aslot)
+    int aslot;
+};
+
+__device__ __forceinline__ RicLane ric_lane(const ConvParams& p, int tid, int ty0, int tx0) {
+    const int wg = tid >> 7, w = (tid >> 5) & 3, l = tid & 31;
+    RicLane ln;
+    ln.r = 64 * wg + 16 * w + (l >> 2);
+    ln.oy = ty0 + (ln.r >> 4);
+    ln.ox = tx0 + (ln.r & 15);
+    ln.live = (ln.oy < p.Hout && ln.ox < p.Wout ? 1u : 0u) | (ln.oy < p.Hout && ln.ox + 8 < p.Wout ? 2u : 0u);
+    // ldmatrix: lanes 0-7 / 8-15 give the rows of matrices 0 / 1 (pixels 0-7 / 8-15 of the warp's tile row, slot 2k),
+    // lanes 16-31 the same pixels for slot 2k + 1
+    const int ra = (ln.r & ~15) + (l & 7) + 8 * ((l >> 3) & 1);
+    ln.ax = tx0 + (ra & 15);
+    ln.aslot = l >> 4;
+    ln.oct = ric_oct(p, ln.r, ty0, tx0) | ric_oct(p, ln.r + 8, ty0, tx0) << 8 | ric_oct(p, ra, ty0, tx0) << 16;
+    return ln;
+}
+
+// Chunk q's A fragments from the block's halo and the tile's stencil: the same corners, entries, blend helpers, centre
+// tap and zero rule as produce_ric_halo, so the fragments hold exactly the values that producer stores.  K-padding slots are
+// zeros in the halo and blend to zeros.
+//   fp16: per corner and K step one ldsm_x4 gathers the corner of each fragment row (every lane gives the row address of
+//   its ldmatrix pixel's corner), then each register is one packed-half2 blend with its row's weights.
+//   Split fp16: K steps 0-1 are the hi and 2-3 the lo parts of the chunk's 32 fp32 channels.  Channels 2t, 2t + 1 (t = l % 4)
+//   of group g sit in halo slot 2g + (t >> 1) at byte 8 (t & 1): one ld.shared.v2 per corner, group and pixel; the blend is
+//   split once, hi into K step g / 2 and lo into g / 2 + 2.
+template <bool kExact>
+__device__ __forceinline__ void build_ric_a(const ConvParams& p, int q, uint32_t halo, uint32_t sten, const RicLane& ln,
+                                            int lane, int ty0, int tx0, uint32_t (*a)[4]) {
+    const int t = q % 9, kq = t < 4 ? t : t - 1;
+    const int hw = ric_halo_cols(p.up), y0 = (ty0 >> p.up) - 1, x0 = (tx0 >> p.up) - 1;
+    auto hpix = [&](int vy, int vx) { return ((vy >> p.up) - y0) * hw + (vx >> p.up) - x0; };
+    auto sector = [&](int j, int& dy0, int& dx0) {     // rotated tap m of pixel j: stencil entry and first corner offset
+        const int m = (kq + (ln.oct >> (8 * j))) & 7;
+        dy0 = ric_r0(m) - 1; dx0 = ric_c0(m) - 1;
+        return m;
+    };
+    if constexpr (!kExact) {
+        auto slot = [&](int hp, int k) { return halo + static_cast<uint32_t>(hp) * 128u + ((static_cast<uint32_t>(2 * k + ln.aslot) ^ static_cast<uint32_t>(hp & 7)) << 4); };
+        if (t == 4) {
+            const int hp = hpix(ln.oy, ln.ax);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) ldsm_x4(a[k], slot(hp, k));
+        } else {
+            int dy0, dx0;
+            sector(2, dy0, dx0);
+            const int vy = ln.oy + dy0, vx = ln.ax + dx0;
+            const int h00 = hpix(vy, vx), h01 = hpix(vy, vx + 1), h10 = hpix(vy + 1, vx), h11 = hpix(vy + 1, vx + 1);
+            RicWeightsH w[2];
+#pragma unroll
+            for (int j = 0; j < 2; ++j) w[j] = ric_weights(ld_shared_v2(sten + static_cast<uint32_t>(sector(j, dy0, dx0) * kTileM + ln.r + 8 * j) * 8u));
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                uint32_t n00[4], n01[4], n10[4], n11[4];
+                ldsm_x4(n00, slot(h00, k)); ldsm_x4(n01, slot(h01, k)); ldsm_x4(n10, slot(h10, k)); ldsm_x4(n11, slot(h11, k));
+#pragma unroll
+                for (int i = 0; i < 4; ++i) a[k][i] = ric_blend(w[i & 1], n00[i], n01[i], n10[i], n11[i]);
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+                if (!((ln.live >> (i & 1)) & 1)) a[k][i] = 0u;
+    } else {
+        // The centre tap and the rotated taps are separate straight-line paths, each issuing all its shared-memory loads
+        // of a pixel before the first blend, so the loads overlap instead of each group waiting for its own.
+        const uint32_t th = static_cast<uint32_t>((lane & 3) >> 1), tb = static_cast<uint32_t>(lane & 1) * 8u;
+        auto ld = [&](int hp, int g) {
+            const uint32_t s = 2u * g + th;
+            const uint2 v = ld_shared_v2(halo + static_cast<uint32_t>(hp) * 128u + ((s ^ static_cast<uint32_t>(hp & 7)) << 4) + tb);
+            return make_float2(__uint_as_float(v.x), __uint_as_float(v.y));
+        };
+        auto put = [&](int j, int g, float2 f) {
+            if (!((ln.live >> j) & 1)) f = make_float2(0.0f, 0.0f);
+            uint32_t hi, lo;
+            split2(f.x, f.y, hi, lo);
+            a[g >> 1][j + 2 * (g & 1)] = hi;
+            a[2 + (g >> 1)][j + 2 * (g & 1)] = lo;
+        };
+        if (t == 4) {
+            float2 v[2][4];
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                const int hp = hpix(ln.oy, ln.ox + 8 * j);
+#pragma unroll
+                for (int g = 0; g < 4; ++g) v[j][g] = ld(hp, g);
+            }
+#pragma unroll
+            for (int j = 0; j < 2; ++j)
+#pragma unroll
+                for (int g = 0; g < 4; ++g) put(j, g, v[j][g]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                int dy0, dx0;
+                const uint2 raw = ld_shared_v2(sten + static_cast<uint32_t>(sector(j, dy0, dx0) * kTileM + ln.r + 8 * j) * 8u);
+                const int vy = ln.oy + dy0, vx = ln.ox + 8 * j + dx0;
+                const int h00 = hpix(vy, vx), h01 = hpix(vy, vx + 1), h10 = hpix(vy + 1, vx), h11 = hpix(vy + 1, vx + 1);
+                float2 v00[4], v01[4], v10[4], v11[4];
+#pragma unroll
+                for (int g = 0; g < 4; ++g) { v00[g] = ld(h00, g); v01[g] = ld(h01, g); v10[g] = ld(h10, g); v11[g] = ld(h11, g); }
+                const RicWeightsF w = ric_weights(make_float2(__uint_as_float(raw.x), __uint_as_float(raw.y)));
+#pragma unroll
+                for (int g = 0; g < 4; ++g)
+                    put(j, g, make_float2(ric_blend(w, v00[g].x, v01[g].x, v10[g].x, v11[g].x),
+                                          ric_blend(w, v00[g].y, v01[g].y, v10[g].y, v11[g].y)));
+            }
+        }
     }
 }
 
@@ -433,7 +600,8 @@ __device__ __forceinline__ void store_tile(const ConvParams& p, uint8_t* smem, c
 // NC = Cout, PN = wgmma N per instruction (a divisor of NC: 32, 64 or 128).  Tap mode reads the split-fp16 K steps from
 // the K masks, so it is instantiated with kExact = false for both precisions.
 //
-// RicHalo mode: the prologue stages the tile's stencil and the halo of channel block 0 (one cp.async group, waited for and
+// RicHalo mode here only for Cout > kRicRegMaxCout (narrower layers run conv_halo_kernel with A in registers): the
+// prologue stages the tile's stencil and the halo of channel block 0 (one cp.async group, waited for and
 // made visible by a barrier before chunk 0 is produced).  Producers run two chunks ahead: chunk c is produced in iteration
 // c - 2 (chunks 0 and 1 in the prologue), so the first chunk of block b (c = 9b) is produced in iteration 9b - 2, and the
 // halo of block b + 1 is issued there, in that iteration's cp.async group.  Block b + 1 is first read by chunk 9b + 9, produced
@@ -443,6 +611,7 @@ __device__ __forceinline__ void store_tile(const ConvParams& p, uint8_t* smem, c
 template <int NC, int PN, ConvMode kMode, bool kExact>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
+    static_assert(!register_a(kMode, NC), "conv_wgmma_kernel: shared-memory A modes only");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_u32 = smem_u32(smem_raw);
     const uint32_t base = (raw_u32 + 1023u) & ~1023u;     // SWIZZLE_128B atoms are 1024-byte aligned
@@ -499,60 +668,82 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     store_tile<NC, 1>(p, smem, s_par, acc, tid, n, ty0, tx0);
 }
 
-// Halo mode.  Chunk q belongs to channel block q / k^2 (every block but the last has exactly k^2 chunks, one per tap; the
-// last one may pack several taps of its few channel groups into a chunk).  Per iteration q: wait for the weight tile of
-// chunk q, issue its MMAs with the A fragments already in registers, wait for the MMAs of chunk q - 1 (their registers
-// are free), ldmatrix the fragments of chunk q + 1, start the weight tile of chunk q + 2 and, in the first iteration of
-// block b, the halo of block b + 1 (it lands k^2 - 2 iterations before it is read; the buffer it overwrites was last
-// read in iteration b k^2 - 2).  The chunk loop is unrolled by two so that the fragment buffers have fixed registers.
-template <int NC, int PN, bool kExact>
-__global__ void __launch_bounds__(kThreads, 1)
+// Halo and RicHalo (Cout <= kRicRegMaxCout) modes.  Chunk q belongs to channel block q / k^2 (every block but the last has
+// exactly k^2 chunks, one per tap; in Halo mode the last one may pack several taps of its few channel groups into a chunk).
+// Per iteration q: wait for the weight tile of chunk q, issue its MMAs with the A fragments already in registers, wait for
+// the MMAs of chunk q - 1 (their registers are free), build the fragments of chunk q + 1, start the weight tile of chunk
+// q + 2 and, in the first iteration of block b, the halo of block b + 1 (it lands k^2 - 2 iterations before it is read; the
+// buffer it overwrites was last read in iteration b k^2 - 2).  The chunk loop is unrolled by two so that the fragment
+// buffers have fixed registers.  The two modes differ only in the fragment source: Halo mode ldmatrix'es each slot's
+// tap-shifted halo pixel (load_a); RicHalo mode blends the rotated tap's corners from the halo with the stencil staged in
+// the prologue (build_ric_a), with 8 x 16 tiles and k^2 = 9 taps per block.  RicHalo layers up to 64 channels run two
+// CTAs per SM (ric_ctas_per_sm) with one fragment buffer, so one CTA's fragment building and barriers overlap the other's
+// MMAs.
+template <int NC, int PN, ConvMode kMode, bool kExact>
+__global__ void __launch_bounds__(kThreads, ric_ctas_per_sm(kMode, NC))
 conv_halo_kernel(const __grid_constant__ ConvParams p) {
-    constexpr int kRows = halo_rows(NC), kM = kRows * kTileW, MB = kM / 128;     // MB: m64 blocks per warpgroup
+    constexpr bool kRic = kMode == ConvMode::RicHalo;
+    static_assert(register_a(kMode, NC), "conv_halo_kernel: Halo, or RicHalo up to kRicRegMaxCout channels");
+    constexpr int kRows = kRic ? kTileH : halo_rows(NC), kM = kRows * kTileW, MB = kM / 128;     // MB: m64 blocks per warpgroup
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_u32 = smem_u32(smem_raw);
     const uint32_t base = (raw_u32 + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base - raw_u32);
-    const SmemLayout L = smem_layout(ConvMode::Halo, NC, p.ksize, 0);
+    const SmemLayout L = smem_layout(kMode, NC, p.ksize, p.up);
     float* s_par = reinterpret_cast<float*>(smem + L.par);
-    const uint32_t zero = base + L.aux;
+    const uint32_t aux = base + L.aux;                    // zero row (Halo) or stencil (RicHalo)
 
     const int tid = threadIdx.x;
     const int wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
     const int n = blockIdx.z;
     const int ty0 = blockIdx.y * kRows;
     const int tx0 = blockIdx.x * kTileW;
-    const int nq = p.nchunks, kk = p.ksize * p.ksize;
+    const int nq = p.nchunks, kk = kRic ? 9 : p.ksize * p.ksize;
     const int hw = kTileW + p.ksize - 1;
 
     load_epilogue_params(p, s_par, tid, kThreads);
-    if (tid < 4) reinterpret_cast<uint32_t*>(smem + L.aux)[tid] = 0u;
+    if (!kRic && tid < 4) reinterpret_cast<uint32_t*>(smem + L.aux)[tid] = 0u;
 
-    // halo pixel of this lane's A row in each m64 block, for the tap (0, 0) of the halo origin
+    // Halo: halo pixel of this lane's A row in each m64 block, for the tap (0, 0) of the halo origin
     int pb[MB];
 #pragma unroll
     for (int mb = 0; mb < MB; ++mb) {
         const int r = wg * (kM / 2) + mb * 64 + warp * 16 + (lane & 15);
         pb[mb] = (r >> 4) * hw + (r & 15);
     }
+    RicLane ln{};
+    if constexpr (kRic) ln = ric_lane(p, tid, ty0, tx0);
     float acc[MB][NC / 2];
 #pragma unroll
     for (int mb = 0; mb < MB; ++mb)
 #pragma unroll
         for (int i = 0; i < NC / 2; ++i) acc[mb][i] = 0.0f;
-    uint32_t a[2][MB][4][4];                              // [buffer][m64 block][K step][register]
+    // [buffer][m64 block][K step][register].  Two-CTA instantiations keep one buffer (128 registers per thread): each
+    // CTA waits for its MMAs before it builds the next chunk, and the other CTA's MMAs fill the gap.
+    constexpr bool kOneBuf = ric_ctas_per_sm(kMode, NC) > 1;
+    uint32_t a[2][MB][4][4];
 
     auto halo_buf = [&](int blk) { return base + L.halo + static_cast<uint32_t>(blk & 1) * L.halo_bytes; };
+    auto load_block = [&](int blk) {
+        if constexpr (kRic) load_ric_halo<kExact>(p, blk, halo_buf(blk), tid, n, ty0, tx0);
+        else load_halo<kRows>(p, blk, halo_buf(blk), tid, n, ty0, tx0);
+    };
+    auto load_frags = [&](int q, uint32_t (*dst)[4][4]) {
+        if constexpr (kRic) build_ric_a<kExact>(p, q, halo_buf(q / kk), aux, ln, lane, ty0, tx0, dst[0]);
+        else load_a<MB>(p, q, halo_buf(q / kk), aux, pb, lane, dst);
+    };
 
-    // prologue: halo of block 0 + weights of chunk 0, then weights of chunk 1 (one cp.async group each)
-    load_halo<kRows>(p, 0, halo_buf(0), tid, n, ty0, tx0);
+    // prologue: (RicHalo: the tile's stencil +) halo of block 0 + weights of chunk 0, then weights of chunk 1 (one
+    // cp.async group each)
+    if constexpr (kRic) stage_ric_stencil<kExact>(p, aux, tid, ty0, tx0);
+    load_block(0);
     produce_b(p, 0, base, tid);
     cp_async_commit();
     if (nq > 1) produce_b(p, 1, base + L.stage_bytes, tid);
     cp_async_commit();
     cp_async_wait<1>();
-    __syncthreads();                                      // halo 0 (and the zero row) visible to every warp
-    load_a<MB>(p, 0, halo_buf(0), zero, pb, lane, a[0]);
+    __syncthreads();                                      // halo 0 (and the zero row or stencil) visible to every warp
+    load_frags(0, a[0]);
 
     auto step = [&](int q, const uint32_t (*cur)[4][4], uint32_t (*nxt)[4][4]) {
         cp_async_wait<kStages - 3>();
@@ -562,16 +753,17 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
         wgmma_fence();
         mma_chunk_rs<NC, PN, MB, kExact>(acc, cur, db);
         wgmma_commit();
-        wgmma_wait<1>();                                  // the MMAs of chunk q - 1 have retired: `nxt` is free
-        if (q + 1 < nq) load_a<MB>(p, q + 1, halo_buf((q + 1) / kk), zero, pb, lane, nxt);
+        if constexpr (kOneBuf) wgmma_wait<0>();           // the MMAs of chunk q have retired: the one buffer is free
+        else wgmma_wait<1>();                             // the MMAs of chunk q - 1 have retired: `nxt` is free
+        if (q + 1 < nq) load_frags(q + 1, nxt);
         if (q + 2 < nq) produce_b(p, q + 2, base + ((q + 2) % kStages) * L.stage_bytes, tid);
         const int blk = q / kk;
-        if (q == blk * kk && blk + 1 < p.nblocks) load_halo<kRows>(p, blk + 1, halo_buf(blk + 1), tid, n, ty0, tx0);
+        if (q == blk * kk && blk + 1 < p.nblocks) load_block(blk + 1);
         cp_async_commit();
     };
     for (int q = 0; q < nq; q += 2) {
-        step(q, a[0], a[1]);
-        if (q + 1 < nq) step(q + 1, a[1], a[0]);
+        step(q, a[0], a[kOneBuf ? 0 : 1]);
+        if (q + 1 < nq) step(q + 1, a[kOneBuf ? 0 : 1], a[0]);
     }
     wgmma_wait<0>();
     cp_async_wait<0>();
@@ -585,16 +777,18 @@ namespace {
 
 template <ConvMode kMode, bool kExact, int NC, int PN>
 cudaError_t launch_one(const ConvParams& p, cudaStream_t stream) {
-    constexpr bool kHalo = kMode == ConvMode::Halo;
-    constexpr int kRows = kHalo ? halo_rows(NC) : kTileH;
+    constexpr int kRows = kMode == ConvMode::Halo ? halo_rows(NC) : kTileH;
     void (*kernel)(ConvParams);
-    if constexpr (kHalo) kernel = conv_halo_kernel<NC, PN, kExact>;
+    if constexpr (register_a(kMode, NC)) kernel = conv_halo_kernel<NC, PN, kMode, kExact>;
     else kernel = conv_wgmma_kernel<NC, PN, kMode, kExact>;
     static bool attr_set[64] = {};                        // the attribute is per function and context: one flag per device
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e == cudaSuccess && !(dev < 64 && attr_set[dev])) {
         e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        // two CTAs per SM need the largest shared-memory carveout of the unified L1 / shared-memory array
+        if (e == cudaSuccess && ric_ctas_per_sm(kMode, NC) > 1)
+            e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         if (e == cudaSuccess && dev < 64) attr_set[dev] = true;
     }
     if (e != cudaSuccess) return e;
