@@ -17,6 +17,9 @@ constexpr int kABytes = kTileM * 128;   // bytes of one A stage
 constexpr int kThreads = 256;   // two warpgroups: producers, MMA issuers and epilogue alike
 constexpr int kStages = 4;      // A + B ring depth; chunk q + 2 is loaded while the MMAs of chunk q run
 constexpr int kMaxSeg = 6;      // concat segments (second half = lo planes in exact mode)
+constexpr int kChannelAlign = 32;   // stored activation widths are multiples of this (the epilogue's 32-column batches)
+// widest output-channel piece of one launch (the widest Cout launch_mode instantiates in that precision)
+constexpr int kMaxPiece(bool exact) { return exact ? 128 : 256; }
 
 // Which mainloop and A producer a convolution launch runs.  This is the one statement of the rule (engine.cu compile_layer
 // records the plan-time mode, conv_mode applies the run-time knobs):
@@ -26,6 +29,13 @@ constexpr int kMaxSeg = 6;      // concat segments (second half = lo planes in e
 //     measured slower on 8 x 16 halo tiles, DESIGN section 7); plan-time knob `halo` (DSU_HALO) = 0 keeps all but conv0 on
 //     Tap, and run-time knob `first` = 0 sends conv0 to Tap.  Every other layer runs Tap.
 // The run-time alternatives use the same chunks and weight packing as the plan-time mode.
+//
+// Output-channel pieces.  Every activation is stored with its width rounded up to a multiple of 32 (kChannelAlign; the
+// padding channels hold exact zeros).  A layer whose padded width exceeds kMaxPiece (128 in split fp16, 256 in fp16) runs as
+// several launches over contiguous channel ranges, widest first (split-fp16 160 -> 128 + 32, fp16 384 -> 256 + 128), each
+// with its own weight tiles, affine and output channel offset; the residual stream and the instance-norm scratch keep the
+// layer's full pitch (EpiParams::resid_pitch).  The mode above is decided once per layer on its padded width, so every piece
+// runs the same mode; only "RicHalo fits" is asked per piece width.
 enum class ConvMode : int {
     Tap,        // conv_wgmma_kernel: each A slot gathered from global memory per (chunk, slot) with cp.async
     Ric,        // conv_wgmma_kernel: stage-1 deformable, the bilinear corners gathered from global memory
@@ -62,7 +72,8 @@ struct EpiParams {
     const float* shift2;
     int act;                // 0 none, 1 ReLU, 2 LeakyReLU(0.2)
     int resid_in, resid_out;
-    float* resid;           // fp32 residual stream [pix][Cout]
+    float* resid;           // fp32 residual stream [pix][resid_pitch], from this launch's first channel
+    int resid_pitch;        // channels per pixel of `resid`: the layer's padded width (> Cout for an output-channel piece)
     ActOut out;             // main output (after residual), ReLU first when out_relu
     ActOut out2;            // second, un-ReLU'd copy (skip connection)
     int out_relu;
@@ -74,6 +85,9 @@ struct EpiParams {
     uint8_t* y_rgba;        // [B,H,W,4] uint8 or null (to_image_space + alpha)
     const uint8_t* alpha_src;   // alpha byte of pixel p at alpha_src[p * alpha_stride]
     int alpha_stride;
+    // one piece of a final layer split into output-channel pieces: the three conv_12 partial dot products of its channels
+    // go to y_part[o][pix] (B*H*W pixels) instead of y_nchw / y_rgba; conv12_tail (frames.cuh) sums the pieces
+    float* y_part;
 };
 
 struct ConvParams {

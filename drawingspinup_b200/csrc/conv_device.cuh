@@ -66,7 +66,7 @@ __device__ __forceinline__ void epilogue_batch(const ConvParams& p, const float*
         }
     }
     if (e.resid_in) {
-        const float4* rp = reinterpret_cast<const float4*>(e.resid + opix * C + cb);
+        const float4* rp = reinterpret_cast<const float4*>(e.resid + opix * e.resid_pitch + cb);
 #pragma unroll
         for (int c = 0; c < 8; ++c) {
             const float4 rv = rp[c];
@@ -74,7 +74,7 @@ __device__ __forceinline__ void epilogue_batch(const ConvParams& p, const float*
         }
     }
     if (e.resid_out) {
-        float4* rp = reinterpret_cast<float4*>(e.resid + opix * C + cb);
+        float4* rp = reinterpret_cast<float4*>(e.resid + opix * e.resid_pitch + cb);
 #pragma unroll
         for (int c = 0; c < 8; ++c) rp[c] = make_float4(f[4 * c], f[4 * c + 1], f[4 * c + 2], f[4 * c + 3]);
     }
@@ -139,7 +139,11 @@ __device__ __forceinline__ void epilogue_row(const ConvParams& p, const float* s
         }
 #undef DSU_EPI_CASE
     }
-    if (tail) {
+    if (tail && e.y_part) {            // one piece of a split conv_12: partial sums only (the final layer is never a sub-pixel class)
+        const size_t npix = static_cast<size_t>(p.B) * p.Hout * p.Wout;
+#pragma unroll
+        for (int o = 0; o < 3; ++o) e.y_part[o * npix + opix] = y3[o];
+    } else if (tail) {
         const size_t plane = static_cast<size_t>(p.Hout) * p.Wout;
         const size_t pin = static_cast<size_t>(oy) * p.Wout + ox;
         uint8_t rgb[3];

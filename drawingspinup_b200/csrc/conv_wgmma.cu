@@ -806,7 +806,7 @@ cudaError_t launch_mode(const ConvParams& p, cudaStream_t stream) {
         case 128: return p.n128 ? launch_one<kMode, kExact, 128, 128>(p, stream) : launch_one<kMode, kExact, 128, 64>(p, stream);
         default: break;
     }
-    if constexpr (!kExact) {              // split-fp16 configurations stop at 128 channels (engine.cu dsu_create)
+    if constexpr (!kExact) {              // split-fp16 launches stop at 128 channels (wider layers run in pieces, conv.cuh kMaxPiece)
         switch (p.Cout) {
             case 160: return launch_one<kMode, kExact, 160, 32>(p, stream);
             case 192: return launch_one<kMode, kExact, 192, 64>(p, stream);

@@ -44,13 +44,17 @@ int fail(int code, const std::string& msg) {
 enum BufId { SK0 = 0, P0, O1, P1, O2, TT, UU, V2, V1, C11, S0, NBUF };
 
 struct SegDef {
-    int buf, choff, nch;   // buffer, first channel, channels consumed (multiple of 8)
+    int buf, choff, nch;   // buffer, first channel, channels consumed (multiple of 8: the stored, padded width)
     int wch0, wn;          // first weight input channel, real weight channels (<= nch)
 };
+
+// stored width of an activation of c channels (conv.cuh: output-channel pieces)
+int padded(int c) { return (c + kChannelAlign - 1) / kChannelAlign * kChannelAlign; }
 
 struct LayerDef {
     std::string name, wkey, bkey, bn, bn2;
     int k = 3, pad = 1, stride = 1, up = 0, ric = 0, cout = 0, level_out = 0;
+    int n0 = 0, nw = 0;    // output-channel piece (conv.cuh): first channel and width of this launch, of the padded(cout) channels
     std::vector<SegDef> segs;
     int act = 0;
     int out_buf = -1, out_choff = 0, out_relu = 0, out2_buf = -1;
@@ -71,12 +75,15 @@ struct LayerDef {
     Slot* d_slots = nullptr;
     Slot* d_hslots = nullptr;  // halo mode: [nblocks][8] channels of each 16-byte slot of a halo pixel
     uint8_t* d_wpack = nullptr;
-    float *d_scale = nullptr, *d_shift = nullptr, *d_scale2 = nullptr, *d_shift2 = nullptr;
+    float *d_scale = nullptr, *d_shift = nullptr, *d_scale2 = nullptr, *d_shift2 = nullptr;   // [nw]: this piece's channels
+    float* d_w12 = nullptr;   // final layer: [3][nw] conv_12 weights of this piece's channels
     double macs_per_px = 0;   // live MACs per output pixel
+    int live() const { return std::min(nw, cout - n0); }   // real (not padding) output channels of the piece
 };
 
 struct Step {
-    int type;    // 0 conv, 1 maxpool, 2 instance norm + activation + stores of layer `layer` (after its last launch)
+    int type;    // 0 conv, 1 maxpool, 2 instance norm + activation + stores of layer `layer` (after its last launch),
+                 // 3 conv_12 of a final layer that ran in pieces (after its last piece)
     int layer;
     int src, src_choff, C, dst;
 };
@@ -145,7 +152,8 @@ struct dsu_engine {
     bool f32_acts = false;    // stage 1 in split-fp16 mode: activation buffers hold fp32 instead of fp16 hi + lo planes
     int buf_level[NBUF]{}, buf_C[NBUF]{};
     bool buf_used[NBUF]{};
-    float *d_w12 = nullptr, *d_b12 = nullptr;
+    float* d_b12 = nullptr;
+    int tail_pieces = 1;      // pieces of the final layer; > 1: its epilogues leave conv_12 partials in tail_part
     // shape-dependent state
     int B = 0, H = 0, W = 0;
     __half* buf_hi[NBUF]{};
@@ -157,6 +165,8 @@ struct dsu_engine {
     float2* inorm_stats = nullptr; // [B][Cmax] (mean, 1/sqrt(var + eps))
     double* inorm_acc = nullptr;   // [B][Cmax][kInormMaxSlices][2] partial sum, sum of squares of each statistics slice
     size_t inorm_cap = 0, inorm_stats_cap = 0;   // bytes of inorm_x, inorm_stats
+    float* tail_part = nullptr;    // [tail_pieces][3][B*H*W] conv_12 partial dot products of the final layer's pieces
+    size_t tail_cap = 0;
     Level lv[3];
     std::map<std::pair<int, int>, std::vector<float>> user_offsets;
     uint8_t *io_color = nullptr, *io_pos = nullptr, *io_edge = nullptr, *io_out = nullptr;
@@ -219,41 +229,56 @@ int build_plan(dsu_engine* E) {
     expect(E, conv12_prefix(c) + ".weight", {3, f[5], 1, 1});
     expect(E, conv12_prefix(c) + ".bias", {3});
 
-    // activation buffers
+    // activation buffers, every width stored padded to a multiple of 32 (x to 8 behind conv0's channels in SK0)
+    int F[6];
+    for (int i = 0; i < 6; ++i) F[i] = padded(f[i]);
     auto setbuf = [&](int b, int level, int C) { E->buf_level[b] = level; E->buf_C[b] = C; E->buf_used[b] = true; };
-    setbuf(SK0, 0, f[0] + cp);
-    setbuf(O1, 1, f[1]);
-    setbuf(O2, 2, f[2]);
-    if (ric) { setbuf(P0, 1, f[0]); setbuf(P1, 2, f[1]); }
-    if (c.resnet_blocks > 0) { setbuf(TT, 2, f[2]); setbuf(UU, 2, f[2]); }
-    setbuf(V2, 1, f[4]);
-    setbuf(V1, 0, f[4]);
-    setbuf(C11, 0, f[5]);
-    if (c.append_smoothers && !ric) setbuf(S0, 0, f[5]);
+    setbuf(SK0, 0, F[0] + cp);
+    setbuf(O1, 1, F[1]);
+    setbuf(O2, 2, F[2]);
+    if (ric) { setbuf(P0, 1, F[0]); setbuf(P1, 2, F[1]); }
+    if (c.resnet_blocks > 0) { setbuf(TT, 2, F[2]); setbuf(UU, 2, F[2]); }
+    setbuf(V2, 1, F[4]);
+    setbuf(V1, 0, F[4]);
+    setbuf(C11, 0, F[5]);
+    if (c.append_smoothers && !ric) setbuf(S0, 0, F[5]);
 
     // in stage 1 the deformable calls pass only .weight, so conv biases are never applied (models.py:302-351)
     auto bias_of = [&](const std::string& p) { return (c.use_bias && !ric) ? p + ".bias" : std::string(); };
-    auto add = [&](LayerDef L) { E->layers.push_back(L); E->steps.push_back(Step{0, (int)E->layers.size() - 1, 0, 0, 0, 0}); };
+    // one launch per output-channel piece, widest first (conv.cuh); a one-piece layer keeps its name, pieces get ".n<i>"
+    const int cap = kMaxPiece(E->exact);
+    auto add = [&](LayerDef L) {
+        const int cpad = padded(L.cout), np = (cpad + cap - 1) / cap;
+        const std::string base = L.name;
+        for (int i = 0; i < np; ++i) {
+            LayerDef P = L;
+            P.n0 = i * cap; P.nw = std::min(cap, cpad - P.n0);
+            if (np > 1) P.name = base + ".n" + std::to_string(i);
+            E->layers.push_back(P);
+            E->steps.push_back(Step{0, (int)E->layers.size() - 1, 0, 0, 0, 0});
+        }
+        if (L.final && np > 1) { E->tail_pieces = np; E->steps.push_back(Step{3, (int)E->layers.size() - 1, 0, 0, 0, 0}); }
+    };
     auto add_norm = [&]() { if (inorm) E->steps.push_back(Step{2, (int)E->layers.size() - 1, 0, 0, 0, 0}); };
     {
         LayerDef L; L.name = "conv0"; L.wkey = "conv0.conv.weight"; L.bkey = bias_of("conv0.conv");
         L.bn = bn ? "conv0.normalization" : ""; L.k = k0; L.pad = k0 / 2; L.ric = ric; L.cout = f[0]; L.level_out = 0;
-        L.segs = {{SK0, f[0], cp, 0, cin}}; L.act = 2; L.out_buf = SK0; L.out_choff = 0; L.inorm = inorm;
+        L.segs = {{SK0, F[0], cp, 0, cin}}; L.act = 2; L.out_buf = SK0; L.out_choff = 0; L.inorm = inorm;
         add(L); add_norm();
     }
-    if (ric) E->steps.push_back(Step{1, -1, SK0, 0, f[0], P0});
+    if (ric) E->steps.push_back(Step{1, -1, SK0, 0, F[0], P0});
     {
         LayerDef L; L.name = "conv1"; L.wkey = "conv1.conv.weight"; L.bkey = bias_of("conv1.conv");
         L.bn = bn ? "conv1.normalization" : ""; L.stride = ric ? 1 : 2; L.ric = ric; L.cout = f[1]; L.level_out = 1;
-        L.segs = {{ric ? P0 : SK0, 0, f[0], 0, f[0]}}; L.act = 2; L.out_buf = O1; L.inorm = inorm;
+        L.segs = {{ric ? P0 : SK0, 0, F[0], 0, f[0]}}; L.act = 2; L.out_buf = O1; L.inorm = inorm;
         add(L); add_norm();
     }
-    if (ric) E->steps.push_back(Step{1, -1, O1, 0, f[1], P1});
+    if (ric) E->steps.push_back(Step{1, -1, O1, 0, F[1], P1});
     const bool has_res = c.resnet_blocks > 0;
     {
         LayerDef L; L.name = "conv2"; L.wkey = "conv2.conv.weight"; L.bkey = bias_of("conv2.conv");
         L.bn = bn ? "conv2.normalization" : ""; L.stride = ric ? 1 : 2; L.ric = ric; L.cout = f[2]; L.level_out = 2;
-        L.segs = {{ric ? P1 : O1, 0, f[1], 0, f[1]}}; L.act = 2;
+        L.segs = {{ric ? P1 : O1, 0, F[1], 0, f[1]}}; L.act = 2;
         if (has_res) { L.out_buf = TT; L.out_relu = 1; L.out2_buf = O2; L.resid_out = 1; }
         else L.out_buf = O2;
         L.inorm = inorm;
@@ -263,11 +288,11 @@ int build_plan(dsu_engine* E) {
         const std::string p = "resnets." + std::to_string(i) + ".";
         LayerDef A; A.name = p + "conv_0"; A.wkey = p + "conv_0.weight"; A.bkey = bias_of(p + "conv_0");
         A.bn = bn ? p + "normalization" : ""; A.ric = ric; A.cout = f[2]; A.level_out = 2;
-        A.segs = {{TT, 0, f[2], 0, f[2]}}; A.act = 1; A.out_buf = UU; A.inorm = inorm;
+        A.segs = {{TT, 0, F[2], 0, f[2]}}; A.act = 1; A.out_buf = UU; A.inorm = inorm;
         add(A); add_norm();
         LayerDef Bl; Bl.name = p + "conv_1"; Bl.wkey = p + "conv_1.weight"; Bl.bkey = bias_of(p + "conv_1");
         Bl.ric = ric; Bl.cout = f[2]; Bl.level_out = 2;
-        Bl.segs = {{UU, 0, f[2], 0, f[2]}}; Bl.act = 0; Bl.resid_in = 1; Bl.resid_out = 1;
+        Bl.segs = {{UU, 0, F[2], 0, f[2]}}; Bl.act = 0; Bl.resid_in = 1; Bl.resid_out = 1;
         Bl.out_buf = TT; Bl.out_relu = (i + 1 < c.resnet_blocks) ? 1 : 0;
         add(Bl);
     }
@@ -289,19 +314,19 @@ int build_plan(dsu_engine* E) {
     {
         LayerDef L; L.name = "upconv2"; L.wkey = "upconv2.1.weight"; L.bn = bn ? "upconv2.2" : "";
         L.ric = ric; L.cout = f[4]; L.level_out = 1;
-        L.segs = {{has_res ? TT : O2, 0, f[2], 0, f[2]}, {O2, 0, f[2], f[3], f[2]}}; L.act = 1; L.out_buf = V2;
+        L.segs = {{has_res ? TT : O2, 0, F[2], 0, f[2]}, {O2, 0, F[2], f[3], f[2]}}; L.act = 1; L.out_buf = V2;
         add_up(L);
     }
     {
         LayerDef L; L.name = "upconv1"; L.wkey = "upconv1.1.weight"; L.bn = bn ? "upconv1.2" : "";
         L.ric = ric; L.cout = f[4]; L.level_out = 0;
-        L.segs = {{V2, 0, f[4], 0, f[4]}, {O1, 0, f[1], f[4], f[1]}}; L.act = 1; L.out_buf = V1;
+        L.segs = {{V2, 0, F[4], 0, f[4]}, {O1, 0, F[1], f[4], f[1]}}; L.act = 1; L.out_buf = V1;
         add_up(L);
     }
     {
         LayerDef L; L.name = "conv_11"; L.wkey = "conv_11.0.weight"; L.bkey = bias_of("conv_11.0");
         L.k = k0; L.pad = k0 / 2; L.ric = ric; L.cout = f[5]; L.level_out = 0;
-        L.segs = {{V1, 0, f[4], 0, f[4]}, {SK0, 0, f[0], f[4], f[0]}, {SK0, f[0], cp, f[4] + f[0], cin}};
+        L.segs = {{V1, 0, F[4], 0, f[4]}, {SK0, 0, F[0], f[4], f[0]}, {SK0, F[0], cp, f[4] + f[0], cin}};
         L.act = 1;
         if (c.append_smoothers) L.out_buf = C11; else L.final = 1;
         add(L);
@@ -310,12 +335,12 @@ int build_plan(dsu_engine* E) {
         if (!ric) {   // stage 1: this conv is dead code (models.py:348-350) and is skipped
             LayerDef L; L.name = "conv_11_a.0"; L.wkey = "conv_11_a.0.weight"; L.bkey = bias_of("conv_11_a.0");
             L.bn2 = "conv_11_a.2"; L.cout = f[5]; L.level_out = 0;
-            L.segs = {{C11, 0, f[5], 0, f[5]}}; L.act = 1; L.out_buf = S0;
+            L.segs = {{C11, 0, F[5], 0, f[5]}}; L.act = 1; L.out_buf = S0;
             add(L);
         }
         LayerDef L; L.name = "conv_11_a.3"; L.wkey = "conv_11_a.3.weight"; L.bkey = bias_of("conv_11_a.3");
         L.ric = ric; L.cout = f[5]; L.level_out = 0;
-        L.segs = {{ric ? C11 : S0, 0, f[5], 0, f[5]}}; L.act = 1; L.final = 1;
+        L.segs = {{ric ? C11 : S0, 0, F[5], 0, f[5]}}; L.act = 1; L.final = 1;
         add(L);
     }
     return DSU_OK;
@@ -375,9 +400,9 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     std::vector<Slot> slots, hslots;
     double real_k = 0;
     for (const SegDef& s : L.segs) real_k += static_cast<double>(s.wn) * k * k;
-    L.macs_per_px = real_k * C;
+    L.macs_per_px = real_k * L.live();
     // algorithmic work of a sub-pixel class = a quarter of the 3x3 layer's output pixels (flops are reported per output pixel of level_out)
-    if (L.sub >= 0) L.macs_per_px = real_k / 4.0 * 9.0 / 4.0 * C;
+    if (L.sub >= 0) L.macs_per_px = real_k / 4.0 * 9.0 / 4.0 * L.live();
     // a sub-pixel class (py, px) pads its 2x2 window by (1 - py, 1 - px) above and left; the slot taps and the halo origin both use it
     L.pad_y = L.sub >= 0 ? 1 - (L.sub >> 1) : L.pad;
     L.pad_x = L.sub >= 0 ? 1 - (L.sub & 1) : L.pad;
@@ -409,10 +434,11 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
         }
     }
     L.first = (!L.ric && L.stride == 1 && L.up == 0 && L.sub < 0 && L.segs.size() == 1 && L.segs[0].nch <= 8 && k > 3 && L.pad == (k - 1) / 2) ? 1 : 0;
-    // Halo mode needs k >= 2: the halo of block b + 1 is loaded in the first chunk of block b and read k^2 - 1 chunks later
+    // Halo mode needs k >= 2: the halo of block b + 1 is loaded in the first chunk of block b and read k^2 - 1 chunks later.
+    // The mode follows the layer's padded width, the same for every piece; whether RicHalo fits, the piece's width.
     L.mode = L.ric ? ConvMode::Ric
-           : (L.stride == 1 && L.up == 0 && k >= 2 && (L.first || (E->knobs.halo && C <= 64))) ? ConvMode::Halo : ConvMode::Tap;
-    L.ric_halo_fits = L.ric && conv_smem_bytes(ConvMode::RicHalo, C, k, L.up) <= 227 * 1024;
+           : (L.stride == 1 && L.up == 0 && k >= 2 && (L.first || (E->knobs.halo && padded(C) <= 64))) ? ConvMode::Halo : ConvMode::Tap;
+    L.ric_halo_fits = L.ric && conv_smem_bytes(ConvMode::RicHalo, L.nw, k, L.up) <= 227 * 1024;
     L.nblocks = L.mode == ConvMode::Tap ? 0 : static_cast<int>(blocks.size());
     if (!L.ric) {
         std::vector<HSlot> all;
@@ -451,7 +477,7 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
         }
     }
     L.nchunks = static_cast<int>(chunks.size());
-    const size_t tile = static_cast<size_t>(C) * 128;
+    const size_t tile = static_cast<size_t>(L.nw) * 128;   // the piece's output channels; rows past cout stay zero
     std::vector<uint8_t> pack(static_cast<size_t>(L.nchunks) * tile, 0);
     size_t off = 0;
     auto put = [&](size_t tile_off, int row, int slot, int ci, __half val) {
@@ -462,11 +488,11 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
         const std::vector<HSlot>& ds = chunks[q];
         const int nd = static_cast<int>(ds.size());
         // B tile(s): row o = output channel, 128 B = 64 K elements, 16-byte slots XOR-swizzled by (row & 7)
-        for (int o = 0; o < C; ++o)
+        for (int o = 0; o < L.live(); ++o)
             for (int d = 0; d < nd; ++d) {
                 const HSlot& h = ds[d];
                 for (int ci = 0; ci < h.nvalid; ++ci) {
-                    const float wv = Wt[((static_cast<size_t>(o) * cin_total + h.wch + ci) * k + h.kh) * k + h.kw];
+                    const float wv = Wt[((static_cast<size_t>(L.n0 + o) * cin_total + h.wch + ci) * k + h.kh) * k + h.kw];
                     const __half wh = __float2half_rn(wv);
                     put(off, o, d, ci, wh);
                     if (exact) put(off, o, d + 4, ci, __float2half_rn(wv - __half2float(wh)));   // [W_hi | W_lo] in one row
@@ -490,7 +516,7 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     if ((rc_up = upload(&L.d_wpack, pack))) return rc_up;
     int rc;
 
-    // epilogue affine: y = act(acc * scale + shift) [* scale2 + shift2]
+    // epilogue affine: y = act(acc * scale + shift) [* scale2 + shift2]; a padding channel gets zeros, so it stores exact zeros
     std::vector<float> scale(C, 1.0f), shift(C, 0.0f), scale2, shift2;
     const std::vector<float>* bias = L.bkey.empty() ? nullptr : &E->w.at(L.bkey);
     auto fold = [&](const std::string& p, std::vector<float>& sc, std::vector<float>& sh) {
@@ -506,10 +532,20 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     if (!L.bn.empty()) fold(L.bn, scale, shift);
     if (bias) for (int i = 0; i < C; ++i) shift[i] += scale[i] * (*bias)[i];
     if (!L.bn2.empty()) fold(L.bn2, scale2, shift2);
-    if ((rc = upload(&L.d_scale, scale))) return rc;
-    if ((rc = upload(&L.d_shift, shift))) return rc;
-    if ((rc = upload(&L.d_scale2, scale2))) return rc;
-    if ((rc = upload(&L.d_shift2, shift2))) return rc;
+    // the piece's channels [n0, n0 + nw) of per-channel vectors with `rows` rows of `stride` channels
+    auto piece = [&](const std::vector<float>& v, int rows, int stride) {
+        std::vector<float> out;
+        if (v.empty()) return out;
+        out.assign(static_cast<size_t>(rows) * L.nw, 0.0f);
+        for (int r = 0; r < rows; ++r)
+            for (int o = 0; o < L.live(); ++o) out[static_cast<size_t>(r) * L.nw + o] = v[static_cast<size_t>(r) * stride + L.n0 + o];
+        return out;
+    };
+    if ((rc = upload(&L.d_scale, piece(scale, 1, C)))) return rc;
+    if ((rc = upload(&L.d_shift, piece(shift, 1, C)))) return rc;
+    if ((rc = upload(&L.d_scale2, piece(scale2, 1, C)))) return rc;
+    if ((rc = upload(&L.d_shift2, piece(shift2, 1, C)))) return rc;
+    if (L.final && (rc = upload(&L.d_w12, piece(E->w.at(conv12_prefix(E->cfg) + ".weight"), 3, C)))) return rc;
     return DSU_OK;
 }
 
@@ -611,9 +647,10 @@ int build_level(dsu_engine* E, Level& lv, int h, int w) {
 struct Workspace {
     size_t hi[NBUF], lo[NBUF];   // activation planes; f32_acts: one fp32 plane behind buf_hi, no lo plane
     size_t resid, inorm_x, inorm_stats, inorm_acc;
+    size_t tail;                 // conv_12 partials of a final layer in pieces
     size_t ric[3];               // the RIC stencil tables of each level (Level: lyx, oct, wh)
     size_t total() const {
-        size_t t = resid + inorm_x + inorm_stats + inorm_acc;
+        size_t t = resid + inorm_x + inorm_stats + inorm_acc + tail;
         for (int b = 0; b < NBUF; ++b) t += hi[b] + lo[b];
         for (int l = 0; l < 3; ++l) t += ric[l];
         return t;
@@ -628,15 +665,17 @@ Workspace workspace(const dsu_engine* E, int B, int H, int W) {
         ws.hi[b] = n * (E->f32_acts ? sizeof(float) : sizeof(__half));
         ws.lo[b] = E->exact && !E->f32_acts ? n * sizeof(__half) : 0;
     }
-    if (E->cfg.resnet_blocks > 0) ws.resid = static_cast<size_t>(B) * (H >> 2) * (W >> 2) * E->cfg.filters[2] * sizeof(float);
+    if (E->cfg.resnet_blocks > 0) ws.resid = static_cast<size_t>(B) * (H >> 2) * (W >> 2) * padded(E->cfg.filters[2]) * sizeof(float);
     int cmax = 0;
     for (const LayerDef& L : E->layers)
         if (L.inorm) {
-            ws.inorm_x = std::max(ws.inorm_x, static_cast<size_t>(B) * (H >> L.level_out) * (W >> L.level_out) * L.cout * sizeof(float));
-            cmax = std::max(cmax, L.cout);
+            const int C = padded(L.cout);
+            ws.inorm_x = std::max(ws.inorm_x, static_cast<size_t>(B) * (H >> L.level_out) * (W >> L.level_out) * C * sizeof(float));
+            cmax = std::max(cmax, C);
         }
     ws.inorm_stats = static_cast<size_t>(B) * cmax * sizeof(float2);
     ws.inorm_acc = static_cast<size_t>(B) * cmax * kInormMaxSlices * 2 * sizeof(double);   // one slot per statistics slice
+    if (E->tail_pieces > 1) ws.tail = static_cast<size_t>(E->tail_pieces) * 3 * B * H * W * sizeof(float);
     if (E->cfg.kind == DSU_KIND_GENERATORJ_RIC)
         for (int l = 0; l < 3; ++l)
             ws.ric[l] = static_cast<size_t>(H >> l) * (W >> l) * (8 * sizeof(float2) + sizeof(uint8_t) + 8 * sizeof(uint2));
@@ -679,6 +718,12 @@ int ensure_shape(dsu_engine* E, int B, int H, int W) {
         CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->inorm_acc), ws.inorm_acc));
         E->inorm_stats_cap = ws.inorm_stats;
     }
+    if (ws.tail > E->tail_cap) {
+        if (E->tail_part) cudaFree(E->tail_part);
+        E->tail_part = nullptr;
+        CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&E->tail_part), ws.tail));
+        E->tail_cap = ws.tail;
+    }
     if (E->cfg.kind == DSU_KIND_GENERATORJ_RIC)
         for (int l = 0; l < 3; ++l) {
             int rc = build_level(E, E->lv[l], H >> l, W >> l);
@@ -715,11 +760,16 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
             continue;
         }
         const LayerDef& L = E->layers[sp.layer];
+        if (sp.type == 3) {
+            CUDA_TRY(conv12_tail(E->tail_part, E->tail_pieces, E->d_b12, E->cfg.tanh, B, H, W, y_dev, y_rgba, alpha_src,
+                                 alpha_stride, st));
+            continue;
+        }
         if (sp.type == 2) {
             // nn.InstanceNorm2d + activation + the stores of layer L's epilogue, from the raw output its launch(es) left in inorm_x
             InstNormApply a{};
             a.x = E->inorm_x; a.stats = E->inorm_stats;
-            a.B = B; a.HW = (H >> L.level_out) * (W >> L.level_out); a.C = L.cout; a.act = L.act;
+            a.B = B; a.HW = (H >> L.level_out) * (W >> L.level_out); a.C = padded(L.cout); a.act = L.act;
             a.resid = L.resid_out ? E->resid : nullptr;
             a.out = act_out(E, L.out_buf, L.out_choff); a.out2 = act_out(E, L.out2_buf, 0); a.out_relu = L.out_relu;
             CUDA_TRY(instance_norm(a, E->inorm_acc, st));
@@ -733,8 +783,8 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
         p.Hin = H >> src_level; p.Win = W >> src_level;
         p.up = L.up; p.Hv = p.Hin << L.up; p.Wv = p.Win << L.up;
         p.mode = conv_mode(E, L); p.stride = L.stride; p.exact = E->exact ? 1 : 0;
-        p.nchunks = L.nchunks; p.nblocks = L.nblocks; p.Cout = L.cout;
-        p.b_bytes = L.cout * 128;
+        p.nchunks = L.nchunks; p.nblocks = L.nblocks; p.Cout = L.nw;
+        p.b_bytes = L.nw * 128;
         p.kmask_full = L.kmask_full; p.kmask_last = L.kmask_last; p.kmask2_full = L.kmask2_full; p.kmask2_last = L.kmask2_last;
         if (L.sub >= 0) { p.sub = 1; p.sub_py = L.sub >> 1; p.sub_px = L.sub & 1; }
         p.ksize = L.k; p.pad_y = L.pad_y; p.pad_x = L.pad_x;
@@ -750,16 +800,22 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
         if (L.ric) { p.ric_lyx = E->lv[L.level_out].lyx; p.ric_oct = E->lv[L.level_out].oct; p.ric_wh = E->lv[L.level_out].wh; }
         EpiParams& e = p.epi;
         e.scale = L.d_scale; e.shift = L.d_shift; e.scale2 = L.d_scale2; e.shift2 = L.d_shift2;
-        e.act = L.act; e.resid_in = L.resid_in; e.resid_out = L.resid_out; e.resid = E->resid;
-        e.out = act_out(E, L.out_buf, L.out_choff); e.out2 = act_out(E, L.out2_buf, 0); e.out_relu = L.out_relu;
+        // a piece stores from its first channel n0; the residual stream and the instance-norm scratch keep the full pitch
+        e.act = L.act; e.resid_in = L.resid_in; e.resid_out = L.resid_out; e.resid = E->resid ? E->resid + L.n0 : nullptr;
+        e.resid_pitch = padded(L.cout);
+        e.out = act_out(E, L.out_buf, L.out_choff + L.n0); e.out2 = act_out(E, L.out2_buf, L.n0); e.out_relu = L.out_relu;
         if (L.inorm) {
             // raw convolution output (+ bias) -> fp32 scratch through the residual-stream store; everything else happens in the type-2 step
-            e.act = 0; e.resid_in = 0; e.resid_out = 1; e.resid = E->inorm_x; e.out_relu = 0;
+            e.act = 0; e.resid_in = 0; e.resid_out = 1; e.resid = E->inorm_x + L.n0; e.out_relu = 0;
             e.out = e.out2 = ActOut{};
         }
         if (L.final) {
-            e.w12 = E->d_w12; e.b12 = E->d_b12; e.tanh_flag = E->cfg.tanh;
-            e.y_nchw = y_dev; e.y_rgba = y_rgba; e.alpha_src = alpha_src; e.alpha_stride = alpha_stride;
+            e.w12 = L.d_w12; e.b12 = E->d_b12; e.tanh_flag = E->cfg.tanh;
+            if (E->tail_pieces > 1) {       // conv_12 partials of this piece; the type-3 step finishes them
+                e.y_part = E->tail_part + static_cast<size_t>(L.n0 / kMaxPiece(E->exact)) * 3 * B * H * W;
+            } else {
+                e.y_nchw = y_dev; e.y_rgba = y_rgba; e.alpha_src = alpha_src; e.alpha_stride = alpha_stride;
+            }
         }
         CUDA_TRY(launch_conv(p, st));
     }
@@ -790,10 +846,10 @@ int dsu_create(const dsu_config* cfg, dsu_handle* out) {
     if (cfg->precision != DSU_PREC_FP16 && cfg->precision != DSU_PREC_FP16X3) return fail(DSU_E_INVALID, "bad precision");
     if (cfg->input_channels < 1 || cfg->input_channels > 16) return fail(DSU_E_INVALID, "input_channels must be in [1,16]");
     if (cfg->resnet_blocks < 0 || cfg->resnet_blocks > 64) return fail(DSU_E_INVALID, "resnet_blocks out of range");
-    const int cmax = cfg->precision == DSU_PREC_FP16X3 ? 128 : 256;
     for (int i = 0; i < 6; ++i)
-        if (cfg->filters[i] < 32 || cfg->filters[i] > cmax || (cfg->filters[i] % 32))
-            return fail(DSU_E_INVALID, "filters must be multiples of 32 in [32," + std::to_string(cmax) + "]");
+        if (cfg->filters[i] < 1 || cfg->filters[i] > 512)
+            return fail(DSU_E_INVALID, "filters[" + std::to_string(i) + "] = " + std::to_string(cfg->filters[i]) +
+                                       ": every width must be in [1, 512]");
     if (cfg->filters[3] != cfg->filters[2])
         return fail(DSU_E_INVALID, "filters[3] must equal filters[2] (upconv2 concatenates the residual trunk, models.py:72)");
     int ndev = 0;
@@ -820,11 +876,11 @@ void dsu_destroy(dsu_handle h) {
     DeviceGuard guard(h->cfg.device);
     for (LayerDef& L : h->layers) {
         cudaFree(L.d_slots); cudaFree(L.d_hslots); cudaFree(L.d_wpack);
-        cudaFree(L.d_scale); cudaFree(L.d_shift); cudaFree(L.d_scale2); cudaFree(L.d_shift2);
+        cudaFree(L.d_scale); cudaFree(L.d_shift); cudaFree(L.d_scale2); cudaFree(L.d_shift2); cudaFree(L.d_w12);
     }
     for (int b = 0; b < NBUF; ++b) { cudaFree(h->buf_hi[b]); cudaFree(h->buf_lo[b]); }
     for (int l = 0; l < 3; ++l) { cudaFree(h->lv[l].lyx); cudaFree(h->lv[l].oct); cudaFree(h->lv[l].wh); }
-    cudaFree(h->resid); cudaFree(h->d_w12); cudaFree(h->d_b12);
+    cudaFree(h->resid); cudaFree(h->d_b12); cudaFree(h->tail_part);
     cudaFree(h->inorm_x); cudaFree(h->inorm_stats); cudaFree(h->inorm_acc);
     cudaFree(h->io_color); cudaFree(h->io_pos); cudaFree(h->io_edge); cudaFree(h->io_out);
     delete h;
@@ -870,7 +926,6 @@ int dsu_finalize(dsu_handle h, void* stream) {
     }
     const std::string p12 = conv12_prefix(h->cfg);
     int rc;
-    if ((rc = upload(&h->d_w12, h->w.at(p12 + ".weight")))) return rc;
     if ((rc = upload(&h->d_b12, h->w.at(p12 + ".bias")))) return rc;
     h->finalized = true;
     return DSU_OK;
@@ -905,7 +960,7 @@ int dsu_forward(dsu_handle h, const float* x_dev, int32_t B, int32_t H, int32_t 
     DEVICE_GUARD(h);
     if ((rc = ensure_shape(h, B, H, W))) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(ingest_f32(x_dev, B, h->cfg.input_channels, h->cin_pad, H, W, act_out(h, SK0, h->cfg.filters[0]), st));
+    CUDA_TRY(ingest_f32(x_dev, B, h->cfg.input_channels, h->cin_pad, H, W, act_out(h, SK0, padded(h->cfg.filters[0])), st));
     return run_network(h, B, H, W, y_dev, nullptr, nullptr, 0, st);
 }
 
@@ -919,7 +974,7 @@ int dsu_forward_u8(dsu_handle h, const uint8_t* color_dev, const uint8_t* pos_de
     DEVICE_GUARD(h);
     if ((rc = ensure_shape(h, B, H, W))) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(ingest_u8(color_dev, pos_dev, edge_dev, h->knobs.derive_edge, B, H, W, act_out(h, SK0, h->cfg.filters[0]), st));
+    CUDA_TRY(ingest_u8(color_dev, pos_dev, edge_dev, h->knobs.derive_edge, B, H, W, act_out(h, SK0, padded(h->cfg.filters[0])), st));
     return run_network(h, B, H, W, y_dev, out_rgba_dev, color_dev + 3, 4, st);
 }
 
@@ -970,7 +1025,7 @@ double dsu_forward_flops(dsu_handle h, int32_t B, int32_t H, int32_t W) {
         if (mp == 0) {   // before finalize: derive from the plan
             double kk = 0;
             for (const SegDef& s : L.segs) kk += s.wn;
-            mp = L.sub >= 0 ? kk * 9.0 / 4.0 * L.cout : kk * L.k * L.k * L.cout;
+            mp = L.sub >= 0 ? kk * 9.0 / 4.0 * L.live() : kk * L.k * L.k * L.live();
         }
         macs += mp * static_cast<double>(H >> L.level_out) * (W >> L.level_out);
     }
@@ -1010,7 +1065,7 @@ int dsu_profile_forward(dsu_handle h, int32_t B, int32_t H, int32_t W, int32_t r
         if (sp.type == 0) {
             const LayerDef& L = h->layers[sp.layer];
             double f = 2.0 * L.macs_per_px * (H >> L.level_out) * (W >> L.level_out) * B;
-            if (L.final) f += 2.0 * 3.0 * L.cout * static_cast<double>(H) * W * B;
+            if (L.final) f += 2.0 * 3.0 * L.live() * static_cast<double>(H) * W * B;
             flops_out[i] = f;
         } else {
             flops_out[i] = 0;
@@ -1022,13 +1077,14 @@ int dsu_profile_forward(dsu_handle h, int32_t B, int32_t H, int32_t W, int32_t r
 const char* dsu_step_name(dsu_handle h, int32_t index) {
     if (!h || index < 0 || index >= static_cast<int>(h->steps.size())) return "";
     const Step& sp = h->steps[index];
-    return sp.type == 0 ? h->layers[sp.layer].name.c_str() : sp.type == 1 ? "maxpool" : "instance_norm";
+    static const char* const kStepNames[] = {"", "maxpool", "instance_norm", "conv_12"};    // Step::type order
+    return sp.type == 0 ? h->layers[sp.layer].name.c_str() : kStepNames[sp.type];
 }
 
 const char* dsu_step_kernel(dsu_handle h, int32_t index) {
     if (!h || index < 0 || index >= static_cast<int>(h->steps.size())) return "";
     const Step& sp = h->steps[index];
-    if (sp.type != 0) return sp.type == 1 ? "maxpool" : "instance_norm";
+    if (sp.type != 0) return dsu_step_name(h, index);
     static const char* const kModeNames[] = {"tap", "ric", "ric_halo", "halo"};    // ConvMode order
     return kModeNames[static_cast<int>(conv_mode(h, h->layers[sp.layer]))];
 }

@@ -114,6 +114,27 @@ __global__ void compose_rgba_kernel(const float* __restrict__ y, const float* __
     out[p] = make_uchar4(to_u8(yp[0]), to_u8(yp[npix_frame]), to_u8(yp[2 * npix_frame]), a);
 }
 
+// conv_12 (+ bias, optional tanh) of a final layer that ran in output-channel pieces: the pieces' partial dot products summed
+// in piece order, then the stores of the fused tail (conv_device.cuh epilogue_row): fp32 NCHW y and / or uint8 RGBA.
+__global__ void conv12_tail_kernel(const float* __restrict__ part, int npieces, const float* __restrict__ b12, int tanh_flag,
+                                   size_t npix_frame, size_t npix, float* __restrict__ y, uchar4* __restrict__ rgba,
+                                   const uint8_t* __restrict__ alpha_src, int alpha_stride) {
+    const size_t p = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
+    if (p >= npix) return;
+    const size_t n = p / npix_frame, r = p % npix_frame;
+    uint8_t rgb[3];
+#pragma unroll
+    for (int o = 0; o < 3; ++o) {
+        float v = 0.0f;
+        for (int k = 0; k < npieces; ++k) v += part[(static_cast<size_t>(k) * 3 + o) * npix + p];
+        v += b12[o];
+        if (tanh_flag) v = tanhf(v);
+        if (y) y[(n * 3 + o) * npix_frame + r] = v;
+        rgb[o] = to_u8(v);
+    }
+    if (rgba) rgba[p] = make_uchar4(rgb[0], rgb[1], rgb[2], alpha_src ? alpha_src[p * alpha_stride] : 255);
+}
+
 // pos2edge (run_render.py:31-57): per channel Sobel-3 (BORDER_REFLECT_101) in float64 on u8/255 with
 // the background (alpha < 255) forced to 2, max magnitude over the 3 channels > 0.3.
 __device__ __forceinline__ bool pos_is_edge(const uchar4* __restrict__ f, int x, int y, int H, int W) {
@@ -286,6 +307,13 @@ cudaError_t overlap_edge(const uint8_t* edge, uint8_t* rgba, size_t npix, cudaSt
 cudaError_t compose_rgba(const float* y, const float* mask, int B, int H, int W, uint8_t* out, cudaStream_t st) {
     const size_t npf = static_cast<size_t>(H) * W, np = npf * B;
     compose_rgba_kernel<<<blocks_for(np, 256), 256, 0, st>>>(y, mask, npf, np, reinterpret_cast<uchar4*>(out));
+    return cudaGetLastError();
+}
+cudaError_t conv12_tail(const float* part, int npieces, const float* b12, int tanh_flag, int B, int H, int W, float* y,
+                        uint8_t* rgba, const uint8_t* alpha_src, int alpha_stride, cudaStream_t st) {
+    const size_t npf = static_cast<size_t>(H) * W, np = npf * B;
+    conv12_tail_kernel<<<blocks_for(np, 256), 256, 0, st>>>(part, npieces, b12, tanh_flag, npf, np, y,
+                                                            reinterpret_cast<uchar4*>(rgba), alpha_src, alpha_stride);
     return cudaGetLastError();
 }
 cudaError_t pos2edge(const uint8_t* pos, int B, int H, int W, uint8_t* edge, cudaStream_t st) {

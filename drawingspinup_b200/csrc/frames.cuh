@@ -21,6 +21,11 @@ cudaError_t to_image_space(const float* x, uint8_t* out, size_t n, cudaStream_t 
 cudaError_t overlap_edge(const uint8_t* edge, uint8_t* rgba, size_t npix, cudaStream_t st);
 cudaError_t compose_rgba(const float* y, const float* mask, int B, int H, int W, uint8_t* out, cudaStream_t st);
 cudaError_t pos2edge(const uint8_t* pos, int B, int H, int W, uint8_t* edge, cudaStream_t st);
+// conv_12 of a final layer split into output-channel pieces: part[piece][3][B*H*W] partial dot products -> sum in piece
+// order + b12 (+ tanh) -> y [B,3,H,W] fp32 and / or rgba [B,H,W,4] (to_u8, alpha byte of pixel p at alpha_src[p *
+// alpha_stride], 255 without alpha_src); either output may be null
+cudaError_t conv12_tail(const float* part, int npieces, const float* b12, int tanh_flag, int B, int H, int W, float* y,
+                        uint8_t* rgba, const uint8_t* alpha_src, int alpha_stride, cudaStream_t st);
 
 // nn.InstanceNorm2d between a convolution (raw fp32 output x[B][HW][C] left by its epilogue) and its activation, followed by
 // the stores the fused epilogue would have done.  Three small launches: statistics (fp64 accumulation), finish, apply.

@@ -49,7 +49,7 @@ typedef struct dsu_engine* dsu_handle;
 typedef struct dsu_config {
     int32_t kind;              /* DSU_KIND_* */
     int32_t input_channels;    /* after the +1 mask +2 pos of test_stage1.py:33-39 (6 in shipped configs) */
-    int32_t filters[6];
+    int32_t filters[6];        /* each in [1, 512]; filters[3] == filters[2] (upconv2 concatenates the trunk) */
     int32_t resnet_blocks;
     int32_t use_bias;
     int32_t tanh;
@@ -119,11 +119,13 @@ double dsu_forward_flops(dsu_handle h, int32_t B, int32_t H, int32_t W);
  * number of launches (<= capacity are written) or a negative error.  Synchronizes the stream. */
 int dsu_profile_forward(dsu_handle h, int32_t B, int32_t H, int32_t W, int32_t reps, void* stream,
                         double* ms_out, double* flops_out, int32_t capacity);
-/* Name of launch i of a forward ("ingest", "conv0", "maxpool", "resnets.3.conv_1", ...). */
+/* Name of launch i of a forward ("ingest", "conv0", "maxpool", "resnets.3.conv_1", ...).  A layer wider than one launch
+ * computes (128 channels in DSU_PREC_FP16X3, 256 in DSU_PREC_FP16) runs as output-channel pieces "<layer>.n0", "<layer>.n1",
+ * ...; a final layer in pieces is followed by "conv_12", which sums their conv_12 partial dot products. */
 const char* dsu_step_name(dsu_handle h, int32_t index);
 /* Mainloop launch i runs with the handle's current plan and knobs: "halo" (A fragments from a shared-memory input halo),
  * "tap" (A tiles gathered per tap), "ric_halo" (stage-1 deformable, stencil and corners from shared memory), "ric" (stage-1
- * deformable, gathered from global memory), or "maxpool" / "instance_norm" for the other steps.  Valid after dsu_finalize. */
+ * deformable, gathered from global memory), or "maxpool" / "instance_norm" / "conv_12" for the other steps.  Valid after dsu_finalize. */
 const char* dsu_step_kernel(dsu_handle h, int32_t index);
 
 /* ---- stand-alone uint8 / fp32 frame steps (device pointers) -------------------------------- */
