@@ -829,6 +829,32 @@ int check_ready(dsu_handle h) {
     return DSU_OK;
 }
 
+// The network input of the uint8 frame path: RGB, then the mask when use_mask, then posXY when use_pos (data.py:36-40), so
+// input_channels = 3 + use_mask + 2 * use_pos (test_stage1.py:33-39, test_stage2.py:37-43) and the checkpoint's input width
+// alone fixes the layout.
+struct FrameLayout {
+    bool mask, pos;
+};
+
+// Checks the arguments of a uint8 frame forward and returns the layout: a NULL pos is allowed exactly when nothing reads it
+int check_frame_args(dsu_handle h, const uint8_t* color, const uint8_t* pos, const uint8_t* out, FrameLayout* layout) {
+    int rc = check_ready(h);
+    if (rc) return rc;
+    const int cin = h->cfg.input_channels;
+    if (cin < 3 || cin > 6)
+        return fail(DSU_E_INVALID, "the uint8 frame path needs input_channels = 3 + use_mask + 2 * use_pos, one of 3, 4, 5, 6 "
+                                   "(RGB | mask | posXY, test_stage1.py:33-39); this handle has " + std::to_string(cin));
+    *layout = FrameLayout{cin == 4 || cin == 6, cin >= 5};
+    if (!color || !out) return fail(DSU_E_INVALID, "null frame pointer");
+    if (!pos && layout->pos)
+        return fail(DSU_E_INVALID, "pos is NULL but input_channels " + std::to_string(cin) + " reads posXY (use_pos); pos may "
+                                   "be NULL only when input_channels is 3 or 4 and derive_edge is off");
+    if (!pos && h->knobs.derive_edge)
+        return fail(DSU_E_INVALID, "pos is NULL but derive_edge is set: derived edges come from the pos frames (pos2edge, "
+                                   "run_render.py:31-57); pos may be NULL only when input_channels is 3 or 4 and derive_edge is off");
+    return DSU_OK;
+}
+
 }  // namespace
 
 // =================================================================== C ABI
@@ -966,23 +992,22 @@ int dsu_forward(dsu_handle h, const float* x_dev, int32_t B, int32_t H, int32_t 
 
 int dsu_forward_u8(dsu_handle h, const uint8_t* color_dev, const uint8_t* pos_dev, const uint8_t* edge_dev,
                    int32_t B, int32_t H, int32_t W, uint8_t* out_rgba_dev, float* y_dev, void* stream) {
-    int rc = check_ready(h);
+    FrameLayout lay;
+    int rc = check_frame_args(h, color_dev, pos_dev, out_rgba_dev, &lay);
     if (rc) return rc;
-    if (!color_dev || !pos_dev || !out_rgba_dev) return fail(DSU_E_INVALID, "null frame pointer");
-    if (h->cfg.input_channels != 6)
-        return fail(DSU_E_INVALID, "the fused uint8 frame path needs input_channels == 6 (RGB + mask + posXY, test_stage1.py:33-39)");
     DEVICE_GUARD(h);
     if ((rc = ensure_shape(h, B, H, W))) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    CUDA_TRY(ingest_u8(color_dev, pos_dev, edge_dev, h->knobs.derive_edge, B, H, W, act_out(h, SK0, padded(h->cfg.filters[0])), st));
+    CUDA_TRY(ingest_u8(color_dev, pos_dev, edge_dev, h->knobs.derive_edge, lay.mask, lay.pos, B, H, W,
+                       act_out(h, SK0, padded(h->cfg.filters[0])), st));
     return run_network(h, B, H, W, y_dev, out_rgba_dev, color_dev + 3, 4, st);
 }
 
 int dsu_forward_u8_host(dsu_handle h, const uint8_t* color_host, const uint8_t* pos_host, const uint8_t* edge_host,
                         int32_t B, int32_t H, int32_t W, uint8_t* out_rgba_host, void* stream) {
-    int rc = check_ready(h);
+    FrameLayout lay;
+    int rc = check_frame_args(h, color_host, pos_host, out_rgba_host, &lay);
     if (rc) return rc;
-    if (!color_host || !pos_host || !out_rgba_host) return fail(DSU_E_INVALID, "null frame pointer");
     DEVICE_GUARD(h);
     const size_t np = static_cast<size_t>(B) * H * W;
     if (np * 4 > h->io_cap) {
@@ -996,9 +1021,10 @@ int dsu_forward_u8_host(dsu_handle h, const uint8_t* color_host, const uint8_t* 
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     CUDA_TRY(cudaMemcpyAsync(h->io_color, color_host, np * 4, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->io_pos, pos_host, np * 4, cudaMemcpyHostToDevice, st));
+    if (pos_host) CUDA_TRY(cudaMemcpyAsync(h->io_pos, pos_host, np * 4, cudaMemcpyHostToDevice, st));
     if (edge_host) CUDA_TRY(cudaMemcpyAsync(h->io_edge, edge_host, np, cudaMemcpyHostToDevice, st));
-    rc = dsu_forward_u8(h, h->io_color, h->io_pos, edge_host ? h->io_edge : nullptr, B, H, W, h->io_out, nullptr, stream);
+    rc = dsu_forward_u8(h, h->io_color, pos_host ? h->io_pos : nullptr, edge_host ? h->io_edge : nullptr, B, H, W, h->io_out,
+                        nullptr, stream);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(out_rgba_host, h->io_out, np * 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));

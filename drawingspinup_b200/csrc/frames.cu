@@ -171,12 +171,14 @@ __global__ void pos2edge_kernel(const uchar4* __restrict__ pos, int B, int H, in
 }
 
 
+// x channels RGB, then the mask when kMask, then posXY when kPos (data.py:36-40); `pos` is read only for kPos or derive_edge
+template <bool kMask, bool kPos>
 __global__ void ingest_u8_kernel(const uchar4* __restrict__ color, const uchar4* __restrict__ pos,
                                  const uint8_t* __restrict__ edge, int derive_edge, int H, int W, size_t npix, ActOut out) {
     const size_t p = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
     if (p >= npix) return;
     uchar4 c = color[p];
-    const uchar4 q = pos[p];
+    const uchar4 q = kPos ? pos[p] : make_uchar4(0, 0, 0, 0);
     const float mask = __fdiv_rn(static_cast<float>(c.w), 255.0f);      // alpha BEFORE the edge burn-in (data.py:28)
     // overlap_edge_on_img: burn where the stored edge map (255 - pos2edge, run_render.py:117-120) is < 255.  derive_edge: no edge
     // map given - the same predicate straight from the pos frame (pos2edge fused into the ingest, nothing crosses PCIe)
@@ -187,7 +189,10 @@ __global__ void ingest_u8_kernel(const uchar4* __restrict__ color, const uchar4*
         burn = pos_is_edge(pos + (p / npf) * npf, static_cast<int>(p % W), static_cast<int>((p / W) % H), H, W);
     }
     if (burn) { c.x = 0; c.y = 0; c.z = 0; }
-    float v[8] = {norm_u8(c.x), norm_u8(c.y), norm_u8(c.z), mask, norm_u8(q.x), norm_u8(q.y), 0.0f, 0.0f};
+    constexpr int kP = kMask ? 4 : 3;                                   // first pos channel
+    float v[8] = {norm_u8(c.x), norm_u8(c.y), norm_u8(c.z), 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
+    if (kMask) v[3] = mask;
+    if (kPos) { v[kP] = norm_u8(q.x); v[kP + 1] = norm_u8(q.y); }
     store_act<8>(out, p, 0, v);
 }
 
@@ -271,11 +276,13 @@ cudaError_t ingest_f32(const float* x, int B, int cin, int cpad, int H, int W, c
     ingest_f32_kernel<<<blocks_for(np, 256), 256, 0, st>>>(x, cin, cpad, npf, np, out);
     return cudaGetLastError();
 }
-cudaError_t ingest_u8(const uint8_t* color, const uint8_t* pos, const uint8_t* edge, int derive_edge, int B, int H, int W,
-                      const ActOut& out, cudaStream_t st) {
+cudaError_t ingest_u8(const uint8_t* color, const uint8_t* pos, const uint8_t* edge, int derive_edge, bool has_mask, bool has_pos,
+                      int B, int H, int W, const ActOut& out, cudaStream_t st) {
     const size_t np = static_cast<size_t>(H) * W * B;
-    ingest_u8_kernel<<<blocks_for(np, 256), 256, 0, st>>>(reinterpret_cast<const uchar4*>(color), reinterpret_cast<const uchar4*>(pos), edge,
-                                                          derive_edge, H, W, np, out);
+    auto kernel = has_mask ? (has_pos ? ingest_u8_kernel<true, true> : ingest_u8_kernel<true, false>)
+                           : (has_pos ? ingest_u8_kernel<false, true> : ingest_u8_kernel<false, false>);
+    kernel<<<blocks_for(np, 256), 256, 0, st>>>(reinterpret_cast<const uchar4*>(color), reinterpret_cast<const uchar4*>(pos), edge,
+                                               derive_edge, H, W, np, out);
     return cudaGetLastError();
 }
 cudaError_t frames_to_tensor(const uint8_t* color, const uint8_t* pos, const uint8_t* edge, int B, int H, int W,

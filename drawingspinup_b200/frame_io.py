@@ -18,6 +18,16 @@ that one call replaces ``test_stage1.py`` + ``test_stage2.py`` + ``gif_writer.py
 PNG decode / encode stay on the host (PIL): at the engine's frame rate they, not the GPU, bound the wall clock
 (``stylize_character`` reports the split), which is why SURVEY.md ranks a GPU codec as the next widening step.
 Multi-GPU: ranks take contiguous frame ranges of every action (``pipeline.shard_range``), each rank writes its own files.
+
+The scripts' ablation flags ``--no_mask`` / ``--no_pos`` (both scripts) and ``--no_edge`` (``test_stage2.py``) select the
+network input layout, the checkpoint folders and the result folders (``layout.py``).  ``--stage 1`` is exactly
+``test_stage1.py [flags]`` and ``--stage 2`` exactly ``test_stage2.py [flags]``, which reads its colour frames from
+``--pre_dir`` (``config_stage2.yaml:61``: ``res_stage1_mask_pos``).  Without ``--stage`` both stages run chained and the
+flags apply to both: stage 2 consumes THIS run's stage-1 frames, ``res_stage1[_mask][_pos]``.  That equals
+``test_stage1.py F; test_stage2.py F`` only when the stage-2 config's ``pre_dir`` names that folder - true for the default
+flags, not for ``--no_mask`` / ``--no_pos``, where the shipped config still reads ``res_stage1_mask_pos``; run ``--stage 1``
+then ``--stage 2 --pre_dir ...`` to reproduce any other pairing.  ``pos/`` and ``edge/`` are not read when no stage uses
+them, so a clip without those folders runs under ``--no_pos`` / ``--no_edge``.
 """
 from __future__ import annotations
 
@@ -32,10 +42,11 @@ import numpy as np
 import torch
 from PIL import Image
 
-STAGE1_LOG = "logs_stage1_mask_pos"            # test_stage1.py:29-39 with the default flags
-STAGE2_LOG = "logs_stage2_mask_pos_edge"       # test_stage2.py:32-48
-STAGE1_RES = STAGE1_LOG.replace("logs", "res")  # test_stage1.py:52
-STAGE2_RES = STAGE2_LOG.replace("logs", "res")  # test_stage2.py:59
+from . import layout
+
+# result folders of the default flags (no --no_* flag); every other name comes from layout.log_name / result_name
+STAGE1_RES, STAGE2_RES = layout.result_name(1), layout.result_name(2)
+STAGE2_PRE_DIR = "res_stage1_mask_pos"          # config_stage2.yaml:61: the folder test_stage2.py reads its colour frames from
 
 
 def list_actions(data_root: str) -> List[str]:
@@ -60,10 +71,11 @@ def _decode(path: str, mode: str) -> np.ndarray:
 
 @dataclass
 class FrameSet:
-    """One clip as uint8 stacks: ``color[F,H,W,4]``, ``pos[F,H,W,4]``, ``edge[F,H,W]`` (None when absent) + file names."""
+    """One clip as uint8 stacks: ``color[F,H,W,4]``, ``pos[F,H,W,4]`` (None when not needed), ``edge[F,H,W]`` (None when
+    absent or not needed) + file names."""
     names: List[str]
     color: torch.Tensor
-    pos: torch.Tensor
+    pos: Optional[torch.Tensor]
     edge: Optional[torch.Tensor]
     decode_seconds: float = 0.0
 
@@ -72,32 +84,40 @@ class FrameSet:
 
     @staticmethod
     def load(action_dir: str, names: Optional[Sequence[str]] = None, need_edge: bool = True, workers: int = 8,
-             pin: Optional[bool] = None) -> "FrameSet":
+             pin: Optional[bool] = None, need_pos: bool = True, color_dir: str = "color") -> "FrameSet":
+        """Decode a clip.  ``color_dir`` is the folder of the colour input (stage 2 alone reads its ``pre_dir``); frame names
+        still come from the ``color/`` listing (data.py:18).  ``pos/`` is not opened without ``need_pos``, ``edge/`` not
+        without ``need_edge``."""
         names = list(list_frames(action_dir) if names is None else names)
         pin = torch.cuda.is_available() if pin is None else pin
         t0 = time.perf_counter()
         if not names:
             z4 = torch.empty((0, 0, 0, 4), dtype=torch.uint8)
-            return FrameSet([], z4, z4.clone(), torch.empty((0, 0, 0), dtype=torch.uint8) if need_edge else None)
-        first = _decode(os.path.join(action_dir, "color", names[0]), "RGBA")
+            return FrameSet([], z4, z4.clone() if need_pos else None,
+                            torch.empty((0, 0, 0), dtype=torch.uint8) if need_edge else None)
+        first = _decode(os.path.join(action_dir, color_dir, names[0]), "RGBA")
         h, w = first.shape[:2]
 
         def alloc(*shape):
             t = torch.empty(shape, dtype=torch.uint8)
             return t.pin_memory() if pin else t
 
-        color, pos = alloc(len(names), h, w, 4), alloc(len(names), h, w, 4)
+        color = alloc(len(names), h, w, 4)
+        pos = alloc(len(names), h, w, 4) if need_pos else None
         have_edge = need_edge and os.path.isdir(os.path.join(action_dir, "edge"))
         edge = alloc(len(names), h, w) if have_edge else None
-        cn, pn = color.numpy(), pos.numpy()
+        cn = color.numpy()
+        pn = pos.numpy() if pos is not None else None
         en = edge.numpy() if edge is not None else None
 
         def one(i: int):
-            c = first if i == 0 else _decode(os.path.join(action_dir, "color", names[i]), "RGBA")
-            p = _decode(os.path.join(action_dir, "pos", names[i]), "RGBA")
-            if c.shape != (h, w, 4) or p.shape != (h, w, 4):
+            c = first if i == 0 else _decode(os.path.join(action_dir, color_dir, names[i]), "RGBA")
+            p = _decode(os.path.join(action_dir, "pos", names[i]), "RGBA") if pn is not None else None
+            if c.shape != (h, w, 4) or (p is not None and p.shape != (h, w, 4)):
                 raise ValueError("%s/%s: frame size differs from the first frame of the clip" % (action_dir, names[i]))
-            cn[i], pn[i] = c, p
+            cn[i] = c
+            if p is not None:
+                pn[i] = p
             if en is not None:
                 e = _decode(os.path.join(action_dir, "edge", names[i]), "L")
                 if e.shape != (h, w):
@@ -141,13 +161,34 @@ def write_gif(frame_dir: str, gif_path: str) -> int:
     return len(files)
 
 
-def load_checkpoints(root_dir: str, uid: str, checkpoint_id: int = 99999):
-    """The two per-character state dicts, on the host (test_stage1.py:45-46, test_stage2.py:51-53)."""
+def load_checkpoints(root_dir: str, uid: str, checkpoint_id: int = 99999, *, stages: Sequence[int] = (1, 2),
+                     use_mask: bool = True, use_pos: bool = True, use_edge: bool = True):
+    """The per-character state dicts ``(stage 1, stage 2)`` on the host, from the checkpoint folders the flags name
+    (test_stage1.py:44-46, test_stage2.py:50-53); None for a stage not in ``stages``."""
     out = []
-    for log in (STAGE1_LOG, STAGE2_LOG):
-        path = os.path.join(root_dir, uid, "mesh", log, "model_%05d.pth" % checkpoint_id)
+    for stage in (1, 2):
+        if stage not in stages:
+            out.append(None)
+            continue
+        path = os.path.join(root_dir, uid, "mesh", layout.log_name(stage, use_mask, use_pos, use_edge),
+                            "model_%05d.pth" % checkpoint_id)
         out.append(torch.load(path, map_location="cpu"))
     return tuple(out)
+
+
+def check_flags(stage: Optional[int] = None, use_edge: bool = True, derive_edge: bool = False, pre_dir: Optional[str] = None,
+                save_alpha: bool = True) -> None:
+    """ValueError for combinations the reference scripts cannot express."""
+    if stage not in (None, 1, 2):
+        raise ValueError("stage must be 1, 2 or None (both chained), got %r" % (stage,))
+    if stage == 1 and not use_edge:
+        raise ValueError("--no_edge is a test_stage2.py flag: stage 1 never burns edges in (test_stage1.py:56)")
+    if stage == 1 and not save_alpha:
+        raise ValueError("--no_alpha is a test_stage2.py flag: test_stage1.py always writes the alpha (test_stage1.py:69-70)")
+    if derive_edge and not use_edge:
+        raise ValueError("derive_edge burns edges found in the pos frames into stage 2's input; --no_edge turns the burn-in off")
+    if pre_dir is not None and stage != 2:
+        raise ValueError("pre_dir is the colour input of stage 2 run alone (--stage 2); chained runs feed this run's stage-1 frames")
 
 
 @dataclass
@@ -167,7 +208,9 @@ def stylize_character(root_dir: str, uid: str, pipeline=None, *, device="cuda:0"
                       checkpoint_id: int = 99999, keep_stage1: bool = True, save_alpha: bool = True, gif: bool = False,
                       rank: int = 0, world: int = 1, workers: int = 8, batch: int = 16,
                       pipeline_factory: Optional[Callable] = None, stack: Optional[bool] = None,
-                      write_png: Optional[bool] = None) -> StylizeReport:
+                      write_png: Optional[bool] = None, stage: Optional[int] = None, use_mask: bool = True,
+                      use_pos: bool = True, use_edge: bool = True, pre_dir: Optional[str] = None,
+                      derive_edge: bool = False) -> StylizeReport:
     """``test_stage1.py --uid U`` + ``test_stage2.py --uid U`` (+ ``gif_writer.py``) in one pass over the character's
     ``mesh/blender_render`` tree.  ``pipeline`` is a ready :class:`StylizationPipeline` (weights already broadcast);
     otherwise the checkpoints are read from the tree.  ``pipeline_factory(sd1, sd2)`` exists for tests of the folder
@@ -175,17 +218,33 @@ def stylize_character(root_dir: str, uid: str, pipeline=None, *, device="cuda:0"
 
     ``stack``: read the clip from its raw frame stacks (``frame_stack.py``: ``<action>/stack/{color,pos,edge}.npy``) instead of
     decoding PNGs, and write the results as stacks too (None = use the stacks of every action that has them).  ``write_png``
-    forces / suppresses the reference's PNG result folders (default: PNGs for PNG inputs, stacks for stack inputs)."""
+    forces / suppresses the reference's PNG result folders (default: PNGs for PNG inputs, stacks for stack inputs).
+
+    ``use_mask`` / ``use_pos`` / ``use_edge`` are the scripts' ``--no_*`` flags (``layout.py``: input layout, checkpoint and
+    result folders).  ``stage=1`` / ``stage=2`` runs that script alone (``keep_stage1`` is then moot); stage 2 alone reads
+    its colour frames from ``pre_dir`` (default ``res_stage1_mask_pos``, config_stage2.yaml:61; in stack mode the layer of
+    that name).  ``derive_edge``: stage 2 finds the edges in the pos frames instead of reading ``edge/``."""
     from . import frame_stack
     from .pipeline import shard_range
+    check_flags(stage, use_edge, derive_edge, pre_dir, save_alpha)
+    runs1, runs2 = stage in (None, 1), stage in (None, 2)
+    color_src = (STAGE2_PRE_DIR if pre_dir is None else pre_dir) if stage == 2 else "color"
+    res1 = layout.result_name(1, use_mask, use_pos)
+    res2 = layout.result_name(2, use_mask, use_pos, use_edge)
     data_root = os.path.join(root_dir, uid, "mesh", "blender_render")
     if pipeline is None:
-        sd1, sd2 = load_checkpoints(root_dir, uid, checkpoint_id)
+        sd1, sd2 = load_checkpoints(root_dir, uid, checkpoint_id, stages=[s for s, r in ((1, runs1), (2, runs2)) if r],
+                                    use_mask=use_mask, use_pos=use_pos, use_edge=use_edge)
         if pipeline_factory is not None:
             pipeline = pipeline_factory(sd1, sd2)
         else:
             from .pipeline import StylizationPipeline
-            pipeline = StylizationPipeline(sd1, sd2, device, precision=precision, batch=batch)
+            pipeline = StylizationPipeline(sd1, sd2, device, precision=precision, batch=batch, derive_edge=derive_edge,
+                                           use_mask=use_mask, use_pos=use_pos, use_edge=use_edge)
+    derive = runs2 and (derive_edge or getattr(pipeline, "derive_edge", False))
+    need_pos = use_pos or derive              # posXY channels, or the frames stage 2 derives its edges from
+    need_edge = runs2 and use_edge
+    keep_stage1 = keep_stage1 and stage is None
     rep = StylizeReport()
     for action in list_actions(data_root):
         adir = os.path.join(data_root, action)
@@ -196,11 +255,11 @@ def stylize_character(root_dir: str, uid: str, pipeline=None, *, device="cuda:0"
             continue
         if use_stack:
             t0 = time.perf_counter()
-            nm, c, p_, e = frame_stack.load_range(adir, lo, hi, need_edge=True)
+            nm, c, p_, e = frame_stack.load_range(adir, lo, hi, need_edge=need_edge, need_pos=need_pos, color_layer=color_src)
             fs = FrameSet(nm, c, p_, e, time.perf_counter() - t0)
         else:
-            fs = FrameSet.load(adir, names[lo:hi], need_edge=True, workers=workers)
-        if fs.edge is None and not getattr(pipeline, "derive_edge", False):
+            fs = FrameSet.load(adir, names[lo:hi], need_edge=need_edge, workers=workers, need_pos=need_pos, color_dir=color_src)
+        if need_edge and fs.edge is None and not derive:
             raise FileNotFoundError(adir + "/edge: stage 2 needs the edge maps (run_render.py:117-120)")
         rep.decode_s += fs.decode_seconds
         out = torch.empty_like(fs.color)
@@ -208,24 +267,25 @@ def stylize_character(root_dir: str, uid: str, pipeline=None, *, device="cuda:0"
         t0 = time.perf_counter()
         mid = pipeline.run_host(fs.color, fs.pos, fs.edge, out, keep_stage1=keep_stage1)
         rep.gpu_s += time.perf_counter() - t0
+        # (result folder, frames, with alpha): test_stage1.py always writes the alpha, test_stage2.py unless --no_alpha
+        layers = ([(res1, mid, True)] if keep_stage1 else []) + [(res2, out, save_alpha) if runs2 else (res1, out, True)]
         png = (not use_stack) if write_png is None else bool(write_png)
         if use_stack:
             t0 = time.perf_counter()
-            if keep_stage1:
-                frame_stack.save_range(adir, STAGE1_RES, mid, lo, len(names))
-            frame_stack.save_range(adir, STAGE2_RES, out, lo, len(names))
+            for res, frames, _ in layers:
+                frame_stack.save_range(adir, res, frames, lo, len(names))
             rep.encode_s += time.perf_counter() - t0
         if png:
-            if keep_stage1:
-                rep.encode_s += save_frames(os.path.join(adir, STAGE1_RES), fs.names, mid, True, workers)
-            rep.encode_s += save_frames(os.path.join(adir, STAGE2_RES), fs.names, out, save_alpha, workers)
+            for res, frames, alpha in layers:
+                rep.encode_s += save_frames(os.path.join(adir, res), fs.names, frames, alpha, workers)
         rep.frames += len(fs)
         rep.actions[action] = len(fs)
     if gif and rank == 0 and world == 1:
-        for action in rep.actions:          # gif_writer.py:13-21 (every action except the rest pose, stage-2 frames)
-            if action != "rest_pose" and os.path.isdir(os.path.join(data_root, action, STAGE2_RES)):
-                write_gif(os.path.join(data_root, action, STAGE2_RES),
-                          os.path.join(data_root, "..", "gif", action + "_" + STAGE2_RES + ".gif"))
+        last = res2 if runs2 else res1      # gif_writer.py:14-16: the res_stage2_* folders, else the res_stage1_* ones
+        for action in rep.actions:          # gif_writer.py:13-21 (every action except the rest pose)
+            if action != "rest_pose" and os.path.isdir(os.path.join(data_root, action, last)):
+                write_gif(os.path.join(data_root, action, last),
+                          os.path.join(data_root, "..", "gif", action + "_" + last + ".gif"))
     return rep
 
 
@@ -235,8 +295,16 @@ def main(argv=None) -> int:
     ap.add_argument("--uid", required=True)
     ap.add_argument("--checkpoint_id", type=int, default=99999)
     ap.add_argument("--precision", default="fp16x3", choices=["fp16", "fp16x3"])
+    ap.add_argument("--stage", type=int, choices=[1, 2], default=None,
+                    help="run test_stage1.py (1) or test_stage2.py (2) alone (default: both, chained)")
+    ap.add_argument("--no_mask", action="store_true", help="checkpoints trained without the mask channel")
+    ap.add_argument("--no_pos", action="store_true", help="checkpoints trained without the posXY channels")
+    ap.add_argument("--no_edge", action="store_true", help="stage 2 trained without the edge burn-in (test_stage2.py only)")
+    ap.add_argument("--pre_dir", default=None,
+                    help="--stage 2: folder (or stack layer) of its colour input (default res_stage1_mask_pos, config_stage2.yaml:61)")
+    ap.add_argument("--derive_edge", action="store_true", help="stage 2 finds the edges in the pos frames instead of reading edge/")
     ap.add_argument("--no_alpha", action="store_true", help="save stage-2 frames without the alpha channel")
-    ap.add_argument("--no_stage1", action="store_true", help="do not write the intermediate res_stage1_mask_pos frames")
+    ap.add_argument("--no_stage1", action="store_true", help="chained run: do not write the intermediate stage-1 frames")
     ap.add_argument("--gif", action="store_true")
     ap.add_argument("--workers", type=int, default=8)
     ap.add_argument("--pack", action="store_true", help="convert every action's PNG tree to raw frame stacks (stack/*.npy) and exit")
@@ -244,6 +312,11 @@ def main(argv=None) -> int:
     ap.add_argument("--png", action="store_true", help="with stacks: also write the reference's PNG result folders")
     ap.add_argument("--unpack", action="store_true", help="write the result stacks out as PNG folders and exit")
     a = ap.parse_args(argv)
+    flags = dict(use_mask=not a.no_mask, use_pos=not a.no_pos, use_edge=not a.no_edge)
+    try:
+        check_flags(a.stage, flags["use_edge"], a.derive_edge, a.pre_dir, not a.no_alpha)
+    except ValueError as e:
+        ap.error(str(e))
     if a.pack or a.unpack:
         from . import frame_stack
         data_root = os.path.join(a.root, a.uid, "mesh", "blender_render")
@@ -252,7 +325,7 @@ def main(argv=None) -> int:
             if a.pack:
                 print("%s: packed %d frames" % (action, frame_stack.pack_action(adir, a.workers)))
             else:
-                for layer in (STAGE1_RES, STAGE2_RES):
+                for layer in (layout.result_name(1, flags["use_mask"], flags["use_pos"]), layout.result_name(2, **flags)):
                     if os.path.isfile(os.path.join(frame_stack.stack_dir(adir), layer + ".npy")):
                         print("%s/%s: %d frames" % (action, layer, frame_stack.unpack_action(adir, layer, None, not a.no_alpha, a.workers)))
         return 0
@@ -260,9 +333,11 @@ def main(argv=None) -> int:
     dev = "cuda:%d" % int(os.environ.get("LOCAL_RANK", "0"))
     rep = stylize_character(a.root, a.uid, device=dev, precision=a.precision, checkpoint_id=a.checkpoint_id,
                             keep_stage1=not a.no_stage1, save_alpha=not a.no_alpha, gif=a.gif, rank=rank, world=world,
-                            workers=a.workers, stack=True if a.stack else None, write_png=True if a.png else None)
-    print("rank %d: %d frames | decode / stack read %.2f s | GPU (H2D + 2 stages + D2H) %.2f s = %.1f frames/s | encode / stack write %.2f s"
-          % (rank, rep.frames, rep.decode_s, rep.gpu_s, rep.gpu_fps, rep.encode_s), flush=True)
+                            workers=a.workers, stack=True if a.stack else None, write_png=True if a.png else None,
+                            stage=a.stage, pre_dir=a.pre_dir, derive_edge=a.derive_edge, **flags)
+    stages = "2 stages" if a.stage is None else "stage %d" % a.stage
+    print("rank %d: %d frames | decode / stack read %.2f s | GPU (H2D + %s + D2H) %.2f s = %.1f frames/s | encode / stack write %.2f s"
+          % (rank, rep.frames, rep.decode_s, stages, rep.gpu_s, rep.gpu_fps, rep.encode_s), flush=True)
     return 0
 
 

@@ -9,7 +9,8 @@ pixels as ONE memory-mappable array per layer:
     <action>/stack/pos.npy        uint8 [F, H, W, 4]
     <action>/stack/edge.npy       uint8 [F, H, W]      optional (stage 2 can derive it from pos: run_render.py:31-57)
     <action>/stack/names.txt      one frame file name per line (NNNN.png), the order of the arrays
-    <action>/stack/res_stage1_mask_pos.npy, res_stage2_mask_pos_edge.npy   uint8 [F, H, W, 4] outputs
+    <action>/stack/res_stage1_mask_pos.npy, res_stage2_mask_pos_edge.npy   uint8 [F, H, W, 4] outputs (named after the
+                                  ablation flags like the reference's result folders: layout.result_name)
 
 ``.npy`` (NumPy format 1.0: 128-byte aligned header + C-order raw bytes) is the container: any tool reads it, ``np.load(...,
 mmap_mode)`` maps it, a rank of a multi-GPU run reads and writes only its own frame range of the same files, and the bytes
@@ -81,14 +82,19 @@ def open_layer(action_dir: str, layer: str, mode: str = "r") -> np.ndarray:
     return np.load(os.path.join(stack_dir(action_dir), layer + ".npy"), mmap_mode=mode)
 
 
-def load_range(action_dir: str, lo: int, hi: int, need_edge: bool = True, pin: Optional[bool] = None):
-    """Frames [lo, hi) of a clip's stacks as (names, color, pos, edge-or-None) host uint8 tensors (pinned when CUDA is there):
-    one memcpy per layer out of the page cache, no decode."""
+def load_range(action_dir: str, lo: int, hi: int, need_edge: bool = True, pin: Optional[bool] = None, need_pos: bool = True,
+               color_layer: str = "color"):
+    """Frames [lo, hi) of a clip's stacks as (names, color, pos-or-None, edge-or-None) host uint8 tensors (pinned when CUDA is
+    there): one memcpy per layer out of the page cache, no decode.  ``color_layer`` is the layer read as the colour input
+    (stage 2 alone reads the stage-1 result layer, its ``pre_dir``); ``pos.npy`` is not opened without ``need_pos``."""
     pin = torch.cuda.is_available() if pin is None else pin
     names = read_names(action_dir)
-    color, pos = open_layer(action_dir, "color"), open_layer(action_dir, "pos")
-    _check(color, "color.npy", 4)
-    _check(pos, "pos.npy", 4, color.shape[:3])
+    color = open_layer(action_dir, color_layer)
+    _check(color, color_layer + ".npy", 4)
+    pos = None
+    if need_pos:
+        pos = open_layer(action_dir, "pos")
+        _check(pos, "pos.npy", 4, color.shape[:3])
     if len(names) != color.shape[0]:
         raise ValueError("%s: names.txt lists %d frames, the stacks hold %d" % (stack_dir(action_dir), len(names), color.shape[0]))
     if not (0 <= lo <= hi <= len(names)):
@@ -105,7 +111,7 @@ def load_range(action_dir: str, lo: int, hi: int, need_edge: bool = True, pin: O
             t.numpy()[...] = mm[lo:hi]
         return t
 
-    return names[lo:hi], take(color), take(pos), (take(edge) if edge is not None else None)
+    return names[lo:hi], take(color), (take(pos) if pos is not None else None), (take(edge) if edge is not None else None)
 
 
 def save_range(action_dir: str, layer: str, frames, lo: int, total: int) -> None:

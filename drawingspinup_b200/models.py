@@ -21,7 +21,7 @@ from typing import Optional, Sequence
 import torch
 import torch.nn as nn
 
-from . import capi
+from . import capi, layout
 
 
 def ric_offsets(height: int, width: int) -> torch.Tensor:
@@ -254,17 +254,32 @@ class _Generator(nn.Module):
         return y
 
     # ------------------------------------------------------------------ fused frame path
-    def forward_frames(self, color: torch.Tensor, pos: torch.Tensor, edge: Optional[torch.Tensor] = None,
+    def _frame_pos(self, pos):
+        """Checks ``pos`` against the input layout (``layout.frame_layout`` of ``input_channels``) before anything launches:
+        it may be None exactly when the layout has no posXY; the C ABI also refuses a None pos while ``derive_edge`` is set."""
+        _, use_pos = layout.frame_layout(self.input_channels)
+        if pos is None and use_pos:
+            raise ValueError("pos is None but input_channels %d reads posXY (use_pos); pos may be None only when "
+                             "input_channels is 3 or 4 and derive_edge is off" % self.input_channels)
+
+    def forward_frames(self, color: torch.Tensor, pos: Optional[torch.Tensor] = None, edge: Optional[torch.Tensor] = None,
                        return_float: bool = False):
         """Device-resident frame loop body of test_stage1.py:60-70 / test_stage2.py:67-78:
         uint8 RGBA colour ``[B,H,W,4]`` + pos ``[B,H,W,4]`` (+ edge ``[B,H,W]`` for stage 2)
-        -> uint8 RGBA result ``[B,H,W,4]`` (and optionally the fp32 network output)."""
+        -> uint8 RGBA result ``[B,H,W,4]`` (and optionally the fp32 network output).  The network input is RGB | mask |
+        posXY as ``input_channels`` says (``layout.py``); ``pos`` may be None when that layout has no posXY and the
+        ``derive_edge`` knob is off."""
         self._check_mode()
+        self._frame_pos(pos)
         for name, t in (("color", color), ("pos", pos)):
-            if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[-1] != 4:
+            if t is not None and (t.dtype != torch.uint8 or t.dim() != 4 or t.shape[-1] != 4):
                 raise RuntimeError("%s must be uint8 [B,H,W,4]" % name)
         handle = self._engine(color.device)
-        color, pos = color.contiguous(), pos.contiguous()
+        color = color.contiguous()
+        pos_p = None
+        if pos is not None:
+            pos = pos.contiguous()
+            pos_p = C.c_void_p(pos.data_ptr())
         b, h, w, _ = color.shape
         self._prepare_shape(h, w)
         out = torch.empty((b, h, w, 4), dtype=torch.uint8, device=color.device)
@@ -275,7 +290,7 @@ class _Generator(nn.Module):
             edge_p = C.c_void_p(edge.data_ptr())
         stream = torch.cuda.current_stream(color.device).cuda_stream
         with torch.cuda.device(color.device):
-            capi.check(capi.lib().dsu_forward_u8(handle, C.c_void_p(color.data_ptr()), C.c_void_p(pos.data_ptr()), edge_p,
+            capi.check(capi.lib().dsu_forward_u8(handle, C.c_void_p(color.data_ptr()), pos_p, edge_p,
                                                  b, h, w, C.c_void_p(out.data_ptr()),
                                                  C.c_void_p(y.data_ptr()) if y is not None else None,
                                                  C.c_void_p(stream)), "dsu_forward_u8")
@@ -283,14 +298,16 @@ class _Generator(nn.Module):
 
     def forward_frames_host(self, color, pos, edge, out, device: torch.device):
         """Same with HOST (ideally pinned) uint8 tensors; copies in, runs, copies the RGBA result
-        into ``out`` and synchronises (C ABI ``dsu_forward_u8_host``)."""
+        into ``out`` and synchronises (C ABI ``dsu_forward_u8_host``).  ``pos`` may be None under the same rule."""
         self._check_mode()
+        self._frame_pos(pos)
         handle = self._engine(device)
         b, h, w, _ = color.shape
         self._prepare_shape(h, w)
         stream = torch.cuda.current_stream(device).cuda_stream
         with torch.cuda.device(device):
-            capi.check(capi.lib().dsu_forward_u8_host(handle, C.c_void_p(color.data_ptr()), C.c_void_p(pos.data_ptr()),
+            capi.check(capi.lib().dsu_forward_u8_host(handle, C.c_void_p(color.data_ptr()),
+                                                      C.c_void_p(pos.data_ptr()) if pos is not None else None,
                                                       C.c_void_p(edge.data_ptr()) if edge is not None else None,
                                                       b, h, w, C.c_void_p(out.data_ptr()), C.c_void_p(stream)),
                        "dsu_forward_u8_host")

@@ -14,6 +14,7 @@ from typing import Dict, Optional, Tuple
 
 import torch
 
+from . import layout
 from .models import GeneratorJ, GeneratorJ_RIC
 
 # generator block of configs/config_stage{1,2}.yaml:5-10 with the +1 mask +2 pos channels of
@@ -83,17 +84,38 @@ def broadcast_state_dict(sd: Optional[Dict[str, torch.Tensor]], src: int = 0, de
 
 
 class StylizationPipeline:
-    """Stage-1 ``GeneratorJ_RIC`` + stage-2 ``GeneratorJ`` of one character on one GPU."""
+    """Stage-1 ``GeneratorJ_RIC`` + stage-2 ``GeneratorJ`` of one character on one GPU.
+
+    ``use_mask`` / ``use_pos`` / ``use_edge`` are the reference's ablation flags (``--no_mask`` / ``--no_pos`` /
+    ``--no_edge``, ``layout.py``): both stages take ``input_channels = 3 + use_mask + 2 * use_pos``; stage 1 never burns
+    edges in (test_stage1.py:56 builds its dataset with ``use_edge=False``), stage 2 only when ``use_edge``.
+    ``sd_stage2=None`` runs stage 1 alone, ``sd_stage1=None`` stage 2 alone (``run`` / ``run_host`` then take the stage-2
+    input RGBA, what ``pre_dir`` holds, as ``color``)."""
 
     def __init__(self, sd_stage1, sd_stage2, device, precision: str = "fp16x3", args: Optional[dict] = None,
-                 batch: int = 16, deterministic: bool = False, derive_edge: bool = False):
+                 batch: int = 16, deterministic: bool = False, derive_edge: bool = False,
+                 use_mask: bool = True, use_pos: bool = True, use_edge: bool = True):
+        if sd_stage1 is None and sd_stage2 is None:
+            raise ValueError("no stage to run: sd_stage1 and sd_stage2 are both None")
+        if derive_edge and not use_edge:
+            raise ValueError("derive_edge=True burns edges into stage 2's input, which use_edge=False (--no_edge) turns off")
         self.device = torch.device(device)
         self.batch = int(batch)
         self.derive_edge = bool(derive_edge) and sd_stage2 is not None
+        self.use_edge = bool(use_edge)
         a = dict(DEFAULT_ARGS if args is None else args)
-        self.g1 = GeneratorJ_RIC(precision=precision, deterministic=deterministic, **a)
-        self.g1.load_state_dict(sd_stage1)
-        self.g1 = self.g1.to(self.device).eval()
+        cin = layout.input_channels(use_mask, use_pos)
+        if args is not None and args.get("input_channels", cin) != cin:
+            raise ValueError("args input_channels=%r contradicts use_mask=%s, use_pos=%s (3 + use_mask + 2 * use_pos = %d)"
+                             % (args["input_channels"], use_mask, use_pos, cin))
+        a["input_channels"] = cin
+        # stage 1 reads pos for posXY; stage 2 also to derive its edges
+        self.reads_pos = bool(use_pos) or self.derive_edge
+        self.g1 = None
+        if sd_stage1 is not None:
+            self.g1 = GeneratorJ_RIC(precision=precision, deterministic=deterministic, **a)
+            self.g1.load_state_dict(sd_stage1)
+            self.g1 = self.g1.to(self.device).eval()
         # sd_stage2 = None: stage 1 only (test_stage1.py alone; BASELINE configs[4]) - run() then returns the stage-1 RGBA
         self.g2 = None
         if sd_stage2 is not None:
@@ -105,31 +127,46 @@ class StylizationPipeline:
                 # fused into the frame-pack kernel); run() / run_host() are then called with edge=None
                 self.g2.set_knob("derive_edge", 1, device=self.device)
 
+    def _inputs(self, pos, edge, keep_stage1):
+        """The pos / edge the stages read (None for what they do not), checked before anything launches."""
+        if pos is None and self.reads_pos:
+            raise ValueError("pos is None but this pipeline reads it (use_pos, or derive_edge in stage 2)")
+        if keep_stage1 and self.g1 is None:
+            raise ValueError("keep_stage1 without stage 1: there is no stage-1 result to keep")
+        return (pos if self.reads_pos else None), (edge if self.g2 is not None and self.use_edge else None)
+
+    def _stages(self, color, pos, edge):
+        r1 = self.g1.forward_frames(color, pos, None) if self.g1 is not None else color
+        return r1, (self.g2.forward_frames(r1, pos, edge) if self.g2 is not None else r1)
+
     @torch.no_grad()
-    def run(self, color: torch.Tensor, pos: torch.Tensor, edge: torch.Tensor, keep_stage1: bool = False):
+    def run(self, color: torch.Tensor, pos: Optional[torch.Tensor] = None, edge: Optional[torch.Tensor] = None,
+            keep_stage1: bool = False):
         """Device uint8 stacks ``color[F,H,W,4]``, ``pos[F,H,W,4]``, ``edge[F,H,W]`` -> stage-2 RGBA
-        ``[F,H,W,4]`` (and the stage-1 RGBA when ``keep_stage1``), ``batch`` frames per launch."""
+        ``[F,H,W,4]`` (and the stage-1 RGBA when ``keep_stage1``), ``batch`` frames per launch.  ``pos`` may be None
+        when no stage reads it; ``edge`` is ignored unless stage 2 runs with ``use_edge``."""
+        pos, edge = self._inputs(pos, edge, keep_stage1)
         n = color.shape[0]
         out = torch.empty_like(color)
         mid = torch.empty_like(color) if keep_stage1 else None
         for lo in range(0, n, self.batch):
             hi = min(n, lo + self.batch)
-            r1 = self.g1.forward_frames(color[lo:hi], pos[lo:hi], None)
-            out[lo:hi] = (self.g2.forward_frames(r1, pos[lo:hi], edge[lo:hi] if edge is not None else None)
-                          if self.g2 is not None else r1)
+            r1, out[lo:hi] = self._stages(color[lo:hi], pos[lo:hi] if pos is not None else None,
+                                          edge[lo:hi] if edge is not None else None)
             if mid is not None:
                 mid[lo:hi] = r1
         return (out, mid) if keep_stage1 else out
 
     @torch.no_grad()
-    def run_host(self, color: torch.Tensor, pos: torch.Tensor, edge: torch.Tensor, out: torch.Tensor,
+    def run_host(self, color: torch.Tensor, pos: Optional[torch.Tensor], edge: Optional[torch.Tensor], out: torch.Tensor,
                  keep_stage1: bool = False):
         """Same from / to HOST (pinned) uint8 stacks: per batch the inputs are copied to the device,
         both stages run, and the stage-2 RGBA result is copied back (``out`` is filled in place).
         Copies run on a second stream so that the upload of batch i+1 and the download of batch i-1
         overlap the kernels of batch i (frames are independent, so this is plain double buffering).
         Returns ``out``; with ``keep_stage1`` the stage-1 RGBA frames (what test_stage1.py writes to
-        ``res_stage1_mask_pos``) are downloaded as well and returned instead."""
+        ``res_stage1_mask_pos``) are downloaded as well and returned instead.  A pos or edge no stage reads is not uploaded."""
+        pos, edge = self._inputs(pos, edge, keep_stage1)
         n = color.shape[0]
         mid = None
         if keep_stage1:
@@ -156,8 +193,7 @@ class StylizationPipeline:
             (c, p, e), ev = nxt
             nxt = upload(spans[i + 1]) if i + 1 < len(spans) else None
             main.wait_event(ev)
-            r1 = self.g1.forward_frames(c, p, None)
-            r2 = self.g2.forward_frames(r1, p, e) if self.g2 is not None else r1
+            r1, r2 = self._stages(c, p, e)
             done = torch.cuda.Event()
             done.record(main)
             with torch.cuda.stream(cs):
@@ -176,12 +212,15 @@ class StylizationPipeline:
         main.synchronize()
         return mid if keep_stage1 else out
 
+    def _stage_models(self):
+        return [g for g in (self.g1, self.g2) if g is not None]
+
     def flops_per_frame(self, h: int, w: int) -> float:
-        return self.g1.algorithmic_flops(1, h, w) + (self.g2.algorithmic_flops(1, h, w) if self.g2 is not None else 0.0)
+        return sum(g.algorithmic_flops(1, h, w) for g in self._stage_models())
 
     def launches_per_batch(self, b: int, h: int, w: int) -> int:
-        return self.g1.kernel_launches(b, h, w) + (self.g2.kernel_launches(b, h, w) if self.g2 is not None else 0)
+        return sum(g.kernel_launches(b, h, w) for g in self._stage_models())
 
     def workspace_bytes(self, b: int, h: int, w: int) -> int:
         """HBM the engine handles hold for a ``b``-frame batch of this size (activations, residual stream, RIC stencils)."""
-        return self.g1.workspace_bytes(b, h, w) + (self.g2.workspace_bytes(b, h, w) if self.g2 is not None else 0)
+        return sum(g.workspace_bytes(b, h, w) for g in self._stage_models())

@@ -98,12 +98,19 @@ int dsu_forward(dsu_handle h, const float* x_dev, int32_t B, int32_t H, int32_t 
  * alpha composite (test_stage1.py:68-70), all on device.
  * color_dev / pos_dev: uint8 RGBA [B,H,W,4]; edge_dev: uint8 [B,H,W] or NULL (stage 2 passes it:
  * overlap_edge_on_img, custom_transforms.py:30-35); out_rgba_dev: uint8 [B,H,W,4];
- * y_dev: optional fp32 NCHW network output (may be NULL). */
+ * y_dev: optional fp32 NCHW network output (may be NULL).
+ * The network input is RGB, then the mask when use_mask, then posXY when use_pos (data.py:36-40), so the handle's
+ * input_channels = 3 + use_mask + 2*use_pos selects it: 3 RGB, 4 RGB|mask, 5 RGB|posXY, 6 RGB|mask|posXY (the
+ * reference's --no_mask / --no_pos ablations).  The output alpha is always the colour alpha.  pos_dev may be NULL exactly
+ * when the layout has no pos (3 or 4) and the derive_edge knob is off.  Any other input_channels, or a NULL pos_dev that
+ * would be read, returns DSU_E_INVALID before any launch. */
 int dsu_forward_u8(dsu_handle h, const uint8_t* color_dev, const uint8_t* pos_dev, const uint8_t* edge_dev,
                    int32_t B, int32_t H, int32_t W, uint8_t* out_rgba_dev, float* y_dev, void* stream);
 
 /* Same as dsu_forward_u8 with HOST buffers (pinned memory recommended): copies the inputs to the
- * device, runs, copies the RGBA result back, and synchronizes the stream before returning. */
+ * device, runs, copies the RGBA result back, and synchronizes the stream before returning.  The same
+ * layouts and rules: pos_host may be NULL exactly when dsu_forward_u8 allows a NULL pos_dev, and is then
+ * not uploaded. */
 int dsu_forward_u8_host(dsu_handle h, const uint8_t* color_host, const uint8_t* pos_host, const uint8_t* edge_host,
                         int32_t B, int32_t H, int32_t W, uint8_t* out_rgba_host, void* stream);
 
@@ -129,8 +136,9 @@ const char* dsu_step_name(dsu_handle h, int32_t index);
 const char* dsu_step_kernel(dsu_handle h, int32_t index);
 
 /* ---- stand-alone uint8 / fp32 frame steps (device pointers) -------------------------------- */
-/* DatasetFullImages.__getitem__ (data.py:23-47): pre_dev fp32 [B,6,H,W] = RGB(3) | mask | posXY(2),
- * mask_dev fp32 [B,1,H,W] (may be NULL).  edge_dev NULL = stage 1. */
+/* DatasetFullImages.__getitem__ (data.py:23-47) in the default layout (use_mask and use_pos):
+ * pre_dev fp32 [B,6,H,W] = RGB(3) | mask | posXY(2), mask_dev fp32 [B,1,H,W] (may be NULL).
+ * edge_dev NULL = stage 1.  The ablation layouts run only inside dsu_forward_u8. */
 int dsu_frames_to_tensor(const uint8_t* color_dev, const uint8_t* pos_dev, const uint8_t* edge_dev,
                          int32_t B, int32_t H, int32_t W, float* pre_dev, float* mask_dev, void* stream);
 /* to_image_space (custom_transforms.py:7-8), n elements. */
