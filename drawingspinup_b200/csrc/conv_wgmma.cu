@@ -21,7 +21,8 @@
 // built from it straight into registers (wgmma RS form, double-buffered across chunks), so an input pixel crosses L2 once
 // per block instead of once per tap, and no A tile passes through shared memory.  Halo mode (halo_rows(Cout) x kTileW
 // patch) reads the fragments with ldmatrix; RicHalo mode (8 x 16 patch) blends them from the rotated tap's corners in
-// the halo with the same helpers as the shared-memory RIC producers.  Weight tiles stream through the same ring as above.
+// the halo with the same helpers as the shared-memory RIC producers.  Weight tiles stream through a ring of bulk copies
+// on mbarriers (one thread issues each tile), and the halos complete on mbarriers too, so the mainloop has no block barrier.
 //
 // After the last chunk both kernels STAGE the accumulators to shared memory as fp32 rows and run the fused epilogue:
 // folded BN / activation / residual, fp16 NHWC (hi [+lo] planes), fp32 activations, the fp32 residual stream, or the
@@ -70,31 +71,49 @@ __host__ __device__ constexpr int ric_ctas_per_sm(ConvMode mode, int cout) {
     return mode == ConvMode::RicHalo && cout <= 64 ? 2 : 1;
 }
 
-// Shared memory from the 1024-aligned base: a ring of kStages stages, then (RicHalo / Halo) two input-halo buffers and the
+// conv_halo_kernel: deepest weight ring (stages) a launch is given when shared memory allows.  Halo mode streams a weight
+// tile per chunk against a few ldmatrix per warp, so it takes up to kMaxRing stages.  RicHalo chunks are bound by building
+// the fragments, and a deeper ring measured slower there (DESIGN section 7), so they keep kStages.
+constexpr int kMaxRing = 8;
+__host__ __device__ constexpr int ring_cap(ConvMode mode) { return mode == ConvMode::Halo ? kMaxRing : kStages; }
+
+// Shared memory from the 1024-aligned base: a ring of `stages` stages, then (RicHalo / Halo) two input-halo buffers and the
 // RicHalo stencil entries ([rotated tap m][tile pixel] x 8 B) or the Halo zero row (16 B, the A rows of K-padding slots), then
-// the epilogue parameters.  The staged fp32 accumulators reuse everything before `par`.
+// the epilogue parameters and (register A) the mbarriers.  The staged fp32 accumulators reuse everything before `par`.
 struct SmemLayout {
+    uint32_t stages;        // ring depth: kStages with A in shared memory; register A: as deep as 227 KB allows, <= ring_cap
     uint32_t stage_bytes;   // A tile + B tile (register A: B tile only)
     uint32_t halo;          // two input halos of halo_bytes each (halo_bytes = 0 in Tap / Ric mode)
     uint32_t halo_bytes;
     uint32_t aux;           // stencil (RicHalo) or zero row (Halo)
     uint32_t par;
+    uint32_t bars;          // register A: full[stages], empty[stages], halo full[2], halo empty[2] (8 B each)
     uint32_t total;
 };
 
-__host__ __device__ inline SmemLayout smem_layout(ConvMode mode, int cout, int ksize, int up) {
+__host__ __device__ inline SmemLayout smem_layout_at(ConvMode mode, int cout, int ksize, int up, int stages) {
     const bool halo = mode == ConvMode::Halo, ric_halo = mode == ConvMode::RicHalo;
     const int rows = halo ? halo_rows(cout) : kTileH;
     SmemLayout L;
+    L.stages = static_cast<uint32_t>(stages);
     L.stage_bytes = (register_a(mode, cout) ? 0u : static_cast<uint32_t>(kABytes)) + static_cast<uint32_t>(cout) * 128u;
-    L.halo = kStages * L.stage_bytes;
+    L.halo = L.stages * L.stage_bytes;
     L.halo_bytes = halo       ? static_cast<uint32_t>((rows + ksize - 1) * (kTileW + ksize - 1)) * 128u
                    : ric_halo ? static_cast<uint32_t>(ric_halo_rows(up) * ric_halo_cols(up)) * 128u : 0u;
     L.aux = L.halo + 2 * L.halo_bytes;
     const uint32_t main_end = L.aux + (halo ? 16u : ric_halo ? kStenBytes : 0u);
     const uint32_t staged = static_cast<uint32_t>(rows * kTileW) * acc_pitch(cout) * 4u;
     L.par = ((main_end > staged ? main_end : staged) + 15u) & ~15u;
-    L.total = L.par + par_bytes(cout);
+    L.bars = L.par + par_bytes(cout);                    // a multiple of 8
+    L.total = L.bars + (register_a(mode, cout) ? (2 * L.stages + 4) * 8u : 0u);
+    return L;
+}
+
+__host__ __device__ inline SmemLayout smem_layout(ConvMode mode, int cout, int ksize, int up) {
+    if (!register_a(mode, cout)) return smem_layout_at(mode, cout, ksize, up, kStages);
+    SmemLayout L = smem_layout_at(mode, cout, ksize, up, ring_cap(mode));
+    for (int s = ring_cap(mode) - 1; s >= kStages && L.total + 1024u > 227u * 1024u; --s)     // conv_smem_bytes <= 227 KB
+        L = smem_layout_at(mode, cout, ksize, up, s);
     return L;
 }
 
@@ -670,11 +689,11 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
 
 // Halo and RicHalo (Cout <= kRicRegMaxCout) modes.  Chunk q belongs to channel block q / k^2 (every block but the last has
 // exactly k^2 chunks, one per tap; in Halo mode the last one may pack several taps of its few channel groups into a chunk).
-// Per iteration q: wait for the weight tile of chunk q, issue its MMAs with the A fragments already in registers, wait for
-// the MMAs of chunk q - 1 (their registers are free), build the fragments of chunk q + 1, start the weight tile of chunk
-// q + 2 and, in the first iteration of block b, the halo of block b + 1 (it lands k^2 - 2 iterations before it is read; the
-// buffer it overwrites was last read in iteration b k^2 - 2).  The chunk loop is unrolled by two so that the fragment
-// buffers have fixed registers.  The two modes differ only in the fragment source: Halo mode ldmatrix'es each slot's
+// The mainloop is an mbarrier pipeline (below, and DESIGN section 4a): weight tiles in a ring of SmemLayout::stages
+// bulk-copied stages, halos with full / empty barriers per buffer, the halo of block b + 1 issued in the first iteration of
+// block b (it lands k^2 - 1 iterations before it is read; the buffer it overwrites was last read in iteration b k^2 - 2).
+// The chunk loop is unrolled by two so that the fragment buffers have fixed registers.  The two modes differ only in the
+// fragment source: Halo mode ldmatrix'es each slot's
 // tap-shifted halo pixel (load_a); RicHalo mode blends the rotated tap's corners from the halo with the stencil staged in
 // the prologue (build_ric_a), with 8 x 16 tiles and k^2 = 9 taps per block.  RicHalo layers up to 64 channels run two
 // CTAs per SM (ric_ctas_per_sm) with one fragment buffer, so one CTA's fragment building and barriers overlap the other's
@@ -717,56 +736,118 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
 #pragma unroll
     for (int mb = 0; mb < MB; ++mb)
 #pragma unroll
-        for (int i = 0; i < NC / 2; ++i) acc[mb][i] = 0.0f;
+        for (int i = 0; i < NC / 2; ++i) acc[mb][i] = pinned_zero();   // not 0.0f: see pinned_zero
     // [buffer][m64 block][K step][register].  Two-CTA instantiations keep one buffer (128 registers per thread): each
     // CTA waits for its MMAs before it builds the next chunk, and the other CTA's MMAs fill the gap.
     constexpr bool kOneBuf = ric_ctas_per_sm(kMode, NC) > 1;
     uint32_t a[2][MB][4][4];
 
+    // mbarriers: full[s] completes when the weight tile in stage s has landed (one arrive with its byte count by the
+    // issuing thread), empty[s] when both warpgroups' MMAs have stopped reading it (one arrive per warpgroup); halo full[i]
+    // when every thread's cp.async of the block in buffer i have landed, halo empty[i] when every warp has built its last
+    // fragments from it (one arrive per warp)
+    const int S = static_cast<int>(L.stages);
+    const uint32_t bars = base + L.bars;
+    auto full_bar = [&](int s) { return bars + 8u * static_cast<uint32_t>(s); };
+    auto empty_bar = [&](int s) { return bars + 8u * static_cast<uint32_t>(S + s); };
+    auto hfull_bar = [&](int blk) { return bars + 8u * static_cast<uint32_t>(2 * S + (blk & 1)); };
+    auto hempty_bar = [&](int blk) { return bars + 8u * static_cast<uint32_t>(2 * S + 2 + (blk & 1)); };
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) {
+            mbar_init(full_bar(s), 1);
+            mbar_init(empty_bar(s), 2);
+        }
+        for (int i = 0; i < 2; ++i) {
+            mbar_init(hfull_bar(i), kThreads);
+            mbar_init(hempty_bar(i), kThreads / 32);
+        }
+        fence_mbar_init();
+    }
+    __syncthreads();                                      // barriers initialised, the zero row written
+
     auto halo_buf = [&](int blk) { return base + L.halo + static_cast<uint32_t>(blk & 1) * L.halo_bytes; };
+    // every thread: its share of block blk's halo, then one arrive on the buffer's full barrier when it has landed
     auto load_block = [&](int blk) {
         if constexpr (kRic) load_ric_halo<kExact>(p, blk, halo_buf(blk), tid, n, ty0, tx0);
         else load_halo<kRows>(p, blk, halo_buf(blk), tid, n, ty0, tx0);
+        cp_async_mbar_arrive(hfull_bar(blk));
     };
-    auto load_frags = [&](int q, uint32_t (*dst)[4][4]) {
-        if constexpr (kRic) build_ric_a<kExact>(p, q, halo_buf(q / kk), aux, ln, lane, ty0, tx0, dst[0]);
-        else load_a<MB>(p, q, halo_buf(q / kk), aux, pb, lane, dst);
+    auto load_frags = [&](int q, int b, uint32_t (*dst)[4][4]) {      // chunk q of channel block b
+        if constexpr (kRic) build_ric_a<kExact>(p, q, halo_buf(b), aux, ln, lane, ty0, tx0, dst[0]);
+        else load_a<MB>(p, q, halo_buf(b), aux, pb, lane, dst);
+    };
+    // thread 0: weight tile of chunk c (one bulk copy) into stage s
+    auto produce_w = [&](int c, int s) {
+        mbar_arrive_expect_tx(full_bar(s), static_cast<uint32_t>(p.b_bytes));
+        bulk_copy_g2s(base + static_cast<uint32_t>(s) * L.stage_bytes, p.wpack + static_cast<size_t>(c) * p.b_bytes,
+                      static_cast<uint32_t>(p.b_bytes), full_bar(s));
     };
 
-    // prologue: (RicHalo: the tile's stencil +) halo of block 0 + weights of chunk 0, then weights of chunk 1 (one
-    // cp.async group each)
+    // prologue: (RicHalo: the tile's stencil with) the halo of block 0, and the weight tiles of chunks 0 .. S - 3
     if constexpr (kRic) stage_ric_stencil<kExact>(p, aux, tid, ty0, tx0);
     load_block(0);
-    produce_b(p, 0, base, tid);
-    cp_async_commit();
-    if (nq > 1) produce_b(p, 1, base + L.stage_bytes, tid);
-    cp_async_commit();
-    cp_async_wait<1>();
-    __syncthreads();                                      // halo 0 (and the zero row or stencil) visible to every warp
-    load_frags(0, a[0]);
+    if (tid == 0)
+        for (int c = 0; c < S - 2 && c < nq; ++c) produce_w(c, c);
+    mbar_wait(hfull_bar(0), 0);
+    load_frags(0, 0, a[0]);
 
+    // Iteration q: wait for the weights of chunk q, issue its MMAs, wait for the MMAs of chunk q - 1 (two buffers) or q (one)
+    // and release that chunk's stage, issue the weights of chunk q + S - 2 into the stage of chunk q - 2 once both
+    // warpgroups released it, build the fragments of chunk q + 1 (waiting for its block's halo if it is the block's first
+    // chunk, releasing the halo after the block's last), and in the first chunk of block b issue the halo of block b + 1
+    // into the buffer block b - 1 used.  No block barrier: the warpgroups meet only at the mbarriers, so one may run a chunk
+    // ahead of the other.  qs / qph: stage and phase parity of chunk q.  Halo mode carries chunk q's channel block and tap
+    // position (k^2 is a run-time value there); RicHalo divides by the constant 9, which keeps two registers free for the
+    // two-CTA instantiations.
+    int qs = 0, cblk = 0, cqt = 0;
+    uint32_t qph = 0;
     auto step = [&](int q, const uint32_t (*cur)[4][4], uint32_t (*nxt)[4][4]) {
-        cp_async_wait<kStages - 3>();
-        fence_proxy_async_smem();
-        __syncthreads();                                  // weights of chunk q landed; the MMAs of chunk q - 2 have retired
-        const uint64_t db = wgmma_desc_sw128(base + (q % kStages) * L.stage_bytes, 1024);
+        mbar_wait(full_bar(qs), qph);
+        const uint64_t db = wgmma_desc_sw128(base + static_cast<uint32_t>(qs) * L.stage_bytes, 1024);
         wgmma_fence();
         mma_chunk_rs<NC, PN, MB, kExact>(acc, cur, db);
         wgmma_commit();
-        if constexpr (kOneBuf) wgmma_wait<0>();           // the MMAs of chunk q have retired: the one buffer is free
-        else wgmma_wait<1>();                             // the MMAs of chunk q - 1 have retired: `nxt` is free
-        if (q + 1 < nq) load_frags(q + 1, nxt);
-        if (q + 2 < nq) produce_b(p, q + 2, base + ((q + 2) % kStages) * L.stage_bytes, tid);
-        const int blk = q / kk;
-        if (q == blk * kk && blk + 1 < p.nblocks) load_block(blk + 1);
-        cp_async_commit();
+        if constexpr (kOneBuf) {
+            wgmma_wait<0>();                              // the MMAs of chunk q have retired: the one buffer is free
+            if ((tid & 127) == 0) mbar_arrive(empty_bar(qs));
+        } else {
+            wgmma_wait<1>();                              // the MMAs of chunk q - 1 have retired: `nxt` is free
+            if (q > 0 && (tid & 127) == 0) mbar_arrive(empty_bar(qs > 0 ? qs - 1 : S - 1));
+        }
+        if (tid == 0 && q + S - 2 < nq) {
+            // chunk q + S - 2 goes to stage (qs - 2) mod S, one round after chunk q - 2 there
+            const int ps = qs >= 2 ? qs - 2 : qs + S - 2;
+            if (q >= 2) mbar_wait(empty_bar(ps), qs >= 2 ? qph : qph ^ 1u);
+            produce_w(q + S - 2, ps);
+        }
+        // chunk q: block blk, tap position qt in it; chunk q + 1: block nb, position nt
+        const int blk = kRic ? q / 9 : cblk, qt = kRic ? q - 9 * blk : cqt;
+        const bool next_blk = qt + 1 == kk;
+        const int nb = next_blk ? blk + 1 : blk, nt = next_blk ? 0 : qt + 1;
+        if (q + 1 < nq) {
+            if (next_blk) mbar_wait(hfull_bar(nb), static_cast<uint32_t>(nb >> 1) & 1u);
+            load_frags(q + 1, nb, nxt);
+            if (nt + 1 == kk || q + 2 == nq) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(hempty_bar(nb));
+            }
+        }
+        if (qt == 0 && blk + 1 < p.nblocks) {
+            if (blk >= 1) mbar_wait(hempty_bar(blk + 1), (static_cast<uint32_t>((blk + 1) >> 1) & 1u) ^ 1u);
+            load_block(blk + 1);
+        }
+        cblk = nb;
+        cqt = nt;
+        if (++qs == S) {
+            qs = 0;
+            qph ^= 1u;
+        }
     };
     for (int q = 0; q < nq; q += 2) {
         step(q, a[0], a[kOneBuf ? 0 : 1]);
         if (q + 1 < nq) step(q + 1, a[kOneBuf ? 0 : 1], a[0]);
     }
     wgmma_wait<0>();
-    cp_async_wait<0>();
     __syncthreads();                                      // ring and halos are free: stage the accumulators over them
     store_tile<NC, MB>(p, smem, s_par, acc, tid, n, ty0, tx0);
 }

@@ -1,5 +1,6 @@
 // Thin inline-PTX wrappers for the sm_90a features the convolution kernels use:
-// cp.async, ldmatrix, proxy fences and warpgroup MMA (wgmma) with shared-memory operand descriptors or A in registers.
+// cp.async, ldmatrix, proxy fences, mbarriers and 1-D bulk copies, and warpgroup MMA (wgmma) with shared-memory operand
+// descriptors or A in registers.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -48,6 +49,39 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
+// ---------------------------------------------------------------- mbarriers (shared-memory, CTA scope)
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+// initialised barriers -> visible to the other threads and to the async proxy (bulk copies complete on them)
+__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.release.cta.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// arrive and add `bytes` to the transaction count the current phase waits for
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.release.cta.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// block until the phase with parity `parity` has completed (try_wait suspends for a while before it returns false)
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+    asm volatile(
+        "{\n\t.reg .pred done;\n"
+        "wait_%=:\n\t"
+        "mbarrier.try_wait.parity.acquire.cta.shared::cta.b64 done, [%0], %1;\n\t"
+        "@!done bra wait_%=;\n\t}" ::"r"(bar), "r"(parity) : "memory");
+}
+// one arrive on `bar` when all of this thread's earlier cp.async have landed; the arrival is one of the count the
+// barrier was initialised with (.noinc)
+__device__ __forceinline__ void cp_async_mbar_arrive(uint32_t bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
+}
+// 1-D bulk copy global -> shared (TMA engine, no tensor map): `bytes` (a multiple of 16, both addresses 16-byte aligned)
+// complete as transactions on `bar`
+__device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+
 // Read-only 128-bit global load under a predicate, zeros otherwise (no branch, no dependence on a dummy address).
 __device__ __forceinline__ uint4 ldg128_if(const void* ptr, bool ok) {
     uint4 v;
@@ -59,6 +93,14 @@ __device__ __forceinline__ uint4 ldg128_if(const void* ptr, bool ok) {
 }
 
 // ---------------------------------------------------------------- wgmma
+// +0.0f from an instruction the compiler keeps in place.  Accumulators zeroed with it stay ahead of the prologue: a plain
+// 0.0f store may be sunk to the mainloop's entry, where ptxas then serialises every wgmma of the loop (C7515).
+__device__ __forceinline__ float pinned_zero() {
+    float z;
+    asm volatile("mov.b32 %0, 0;" : "=f"(z));
+    return z;
+}
+
 // Shared-memory matrix descriptor, K-major operand, 128-byte swizzle: rows of 128 B (64 fp16 of K), 8-row groups
 // `sbo_bytes` apart, the 16-byte chunk c of row r at r * 128 + ((c ^ (r & 7)) << 4) inside a 1024-byte aligned atom.
 // Adding 2 to the descriptor (32 bytes) steps to the next K16 slice of the row.
