@@ -23,8 +23,7 @@ constexpr int kMaxPiece(bool exact) { return exact ? 128 : 256; }
 
 // Which mainloop and A producer a convolution launch runs.  This is the one statement of the rule (engine.cu compile_layer
 // records the plan-time mode, conv_mode applies the run-time knobs):
-//   * stage-1 (RIC) layers run RicHalo where its shared-memory layout fits 227 KB (every split-fp16 layer; in fp16 not Cout >= 224
-//     without fused upsampling), else Ric.  Knob `ric_halo` = 0 keeps them all on Ric.
+//   * stage-1 (RIC) layers run RicHalo; knob `ric_halo` = 0 keeps them on Ric.
 //   * a stage-2 layer runs Halo when it is stride 1 without fused upsampling and either conv0-shaped or Cout <= 64 (wider layers
 //     measured slower on 8 x 16 halo tiles, DESIGN section 7); plan-time knob `halo` (DSU_HALO) = 0 keeps all but conv0 on
 //     Tap, and run-time knob `first` = 0 sends conv0 to Tap.  Every other layer runs Tap.
@@ -35,13 +34,12 @@ constexpr int kMaxPiece(bool exact) { return exact ? 128 : 256; }
 // several launches over contiguous channel ranges, widest first (split-fp16 160 -> 128 + 32, fp16 384 -> 256 + 128), each
 // with its own weight tiles, affine and output channel offset; the residual stream and the instance-norm scratch keep the
 // layer's full pitch (EpiParams::resid_pitch).  The mode above is decided once per layer on its padded width, so every piece
-// runs the same mode; only "RicHalo fits" is asked per piece width.
+// runs the same mode.
 enum class ConvMode : int {
     Tap,        // conv_wgmma_kernel: each A slot gathered from global memory per (chunk, slot) with cp.async
     Ric,        // conv_wgmma_kernel: stage-1 deformable, the bilinear corners gathered from global memory
-    RicHalo,    // stage-1 deformable, stencil and corners staged in shared memory: conv_halo_kernel blending the A fragments
-                // straight into registers for Cout <= 128 (every split-fp16 layer), conv_wgmma_kernel with a shared-memory
-                // A ring above (fp16 only)
+    RicHalo,    // conv_halo_kernel at every width: stage-1 deformable, stencil and corners staged in shared memory, the A
+                // fragments blended straight into registers
     Halo,       // conv_halo_kernel: stride 1, A fragments read with ldmatrix from a shared-memory input halo
 };
 
@@ -124,6 +122,5 @@ struct ConvParams {
 };
 
 cudaError_t launch_conv(const ConvParams& p, cudaStream_t stream);
-size_t conv_smem_bytes(ConvMode mode, int cout, int ksize, int up);
 
 }  // namespace dsu

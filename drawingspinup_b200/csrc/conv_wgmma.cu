@@ -1,28 +1,28 @@
 // Fused convolution as an implicit GEMM on the Hopper tensor cores (wgmma, fp32 accumulators in registers).
 //
 // One CTA computes a tile of output pixels (GEMM M) of one frame for all Cout channels (GEMM N), K = taps x input
-// channels walked in 64-element chunks.  Two warpgroups (256 threads) do everything in turn.  Two mainloops:
+// channels walked in 64-element chunks.  Two warpgroups (256 threads) do everything in turn.  Two mainloops, one per
+// source of the A operand:
 //
-// conv_wgmma_kernel (Tap, Ric modes, and RicHalo for Cout > kRicRegMaxCout): a kTileH x kTileW patch (128 pixels).  Each
-// chunk goes through a kStages-deep ring of shared-memory stages holding the A operand (one 128-byte SWIZZLE_128B row per
-// output pixel) and the chunk's pre-swizzled weight tile (B operand, one 128-byte row per output channel).
+// conv_wgmma_kernel (Tap and Ric modes: A from global memory): a kTileH x kTileW patch (128 pixels).  Each chunk goes
+// through a kStages-deep ring of shared-memory stages holding the A operand (one 128-byte SWIZZLE_128B row per output
+// pixel) and the chunk's pre-swizzled weight tile (B operand, one 128-byte row per output channel).
 //   * PRODUCE chunk q + 2 while the MMAs of chunk q run.  Tap mode: each 16-byte slot of an A row is 8 channels of one
 //     tap of one concat segment (slot table), so stride 2 and fused nearest-x2 upsampling are pure address arithmetic
-//     (cp.async with zero fill at the border).  RIC (stage-1 deformable) layers blend the four bilinear corners of the
-//     rotated tap in registers and store the result; the corners come either straight from global memory (Ric, the gather
-//     producer) or, in RicHalo mode, from the channel block's input halo (the tile +- 1 source pixel, staged once per
-//     block with cp.async, double-buffered) with the tile's stencil staged once per CTA.  The weight tile is streamed
-//     with cp.async.
+//     (cp.async with zero fill at the border).  Ric mode (stage-1 deformable layers, the gather producer) loads the four
+//     bilinear corners of the rotated tap straight from global memory, blends them in registers and stores the result.
+//     The weight tile is streamed with cp.async.
 //   * ISSUE wgmma: warpgroup w multiplies A rows 64w .. 64w+63 by the whole weight tile into its register accumulators.
 //
-// conv_halo_kernel (Halo mode, and RicHalo for Cout <= kRicRegMaxCout): the concat is walked in channel blocks of 128 bytes
-// per pixel (8 groups of 8 channels, or 4 groups as hi + lo in exact mode).  The tile's input halo of a block is loaded
-// once with cp.async (double-buffered: block b + 1 lands while the taps of block b run) and every chunk's A fragments are
-// built from it straight into registers (wgmma RS form, double-buffered across chunks), so an input pixel crosses L2 once
-// per block instead of once per tap, and no A tile passes through shared memory.  Halo mode (halo_rows(Cout) x kTileW
-// patch) reads the fragments with ldmatrix; RicHalo mode (8 x 16 patch) blends them from the rotated tap's corners in
-// the halo with the same helpers as the shared-memory RIC producers.  Weight tiles stream through a ring of bulk copies
-// on mbarriers (one thread issues each tile), and the halos complete on mbarriers too, so the mainloop has no block barrier.
+// conv_halo_kernel (Halo and RicHalo modes: A from a shared-memory input halo): the concat is walked in channel blocks of
+// 128 bytes per pixel (8 groups of 8 channels, or 4 groups as hi + lo in exact mode).  The tile's input halo of a block is
+// loaded once with cp.async (double-buffered: block b + 1 lands while the taps of block b run) and every chunk's A
+// fragments are built from it straight into registers (wgmma RS form, double-buffered across chunks), so an input pixel
+// crosses L2 once per block instead of once per tap, and no A tile passes through shared memory.  Halo mode
+// (halo_rows(Cout) x kTileW patch) reads the fragments with ldmatrix; RicHalo mode (8 x 16 patch: the tile +- 1 source
+// pixel per block, with the tile's stencil staged once per CTA) blends them from the rotated tap's corners in the halo
+// with the same helpers as the gather producer.  Weight tiles stream through a ring of bulk copies on mbarriers (one
+// thread issues each tile), and the halos complete on mbarriers too, so the mainloop has no block barrier.
 //
 // After the last chunk both kernels STAGE the accumulators to shared memory as fp32 rows and run the fused epilogue:
 // folded BN / activation / residual, fp16 NHWC (hi [+lo] planes), fp32 activations, the fp32 residual stream, or the
@@ -36,37 +36,29 @@ namespace dsu {
 
 namespace {
 
-__host__ __device__ inline uint32_t acc_pitch(int cout) { return static_cast<uint32_t>(cout) + 4; }   // floats per staged row
+__host__ __device__ constexpr uint32_t acc_pitch(int cout) { return static_cast<uint32_t>(cout) + 4; }   // floats per staged row
 
-__host__ __device__ inline uint32_t par_bytes(int cout) { return (7 * cout + 4) * 4; }
+__host__ __device__ constexpr uint32_t par_bytes(int cout) { return (7 * cout + 4) * 4; }
 
 // RicHalo mode: every corner of the 3 x 3 neighbourhoods of a tile lies in source rows (ty0 >> up) - 1 .. ((ty0 + kTileH) >> up)
 // and columns (tx0 >> up) - 1 .. ((tx0 + kTileW) >> up): 10 x 18 pixels at up = 0, 6 x 10 with the fused nearest x2
-__host__ __device__ inline int ric_halo_rows(int up) { return (kTileH >> up) + 2; }
-__host__ __device__ inline int ric_halo_cols(int up) { return (kTileW >> up) + 2; }
+__host__ __device__ constexpr int ric_halo_rows(int up) { return (kTileH >> up) + 2; }
+__host__ __device__ constexpr int ric_halo_cols(int up) { return (kTileW >> up) + 2; }
 constexpr uint32_t kStenBytes = kTileM * 8 * 8;
 
 // Halo mode: output rows per tile.  16 x 16 tiles halve the weight traffic per pixel; above 64 channels the two m64 blocks
 // per warpgroup would not fit the register file next to the accumulators, so those layers keep 8 x 16.
 __host__ __device__ constexpr int halo_rows(int cout) { return cout <= 64 ? 16 : 8; }
 
-// RicHalo mode: layers up to this width build their A fragments in registers (conv_halo_kernel); that covers every
-// split-fp16 layer (those configurations stop at 128 channels) and every layer of the default network.  Wider fp16 layers
-// keep the shared-memory A ring of conv_wgmma_kernel and its layout, so which of them fit the RicHalo layout at all
-// (engine.cu ric_halo_fits) is unchanged.  Compiled on the register path they would need 186-234 registers, without
-// spills, but they have not been measured there.
-constexpr int kRicRegMaxCout = 128;
+// whether a launch of this mode runs conv_halo_kernel (A fragments built in registers from a shared-memory input halo)
+// rather than conv_wgmma_kernel (A tiles gathered from global memory into a shared-memory ring)
+__host__ __device__ constexpr bool uses_halo_kernel(ConvMode mode) { return mode == ConvMode::Halo || mode == ConvMode::RicHalo; }
 
-// whether a launch of this mode and width takes its A operand from registers (conv_halo_kernel)
-__host__ __device__ constexpr bool register_a(ConvMode mode, int cout) {
-    return mode == ConvMode::Halo || (mode == ConvMode::RicHalo && cout <= kRicRegMaxCout);
-}
-
-// CTAs per SM a conv_halo_kernel instantiation is built for.  A RicHalo CTA with A in registers spends most of each chunk
-// building the next chunk's fragments and at its barrier, with only two warps per SM sub-partition to hide the
-// shared-memory latency, so the tensor cores idle.  Up to 64 channels a second CTA fits: <= 128 registers per thread
-// (launch bounds; ptxas keeps two 8-byte values in a 16-byte stack slot) and <= 90 KB of shared memory each (ring
-// 4 x 8 KB, two 22.5 KB halos, 8 KB stencil, parameters).
+// CTAs per SM a conv_halo_kernel instantiation is built for.  A RicHalo CTA spends most of each chunk building the next
+// chunk's fragments and at its barrier, with only two warps per SM sub-partition to hide the shared-memory latency, so the
+// tensor cores idle.  Up to 64 channels a second CTA fits: <= 128 registers per thread (launch bounds; ptxas keeps two
+// 8-byte values in a 16-byte stack slot) and <= 90 KB of shared memory each (ring 4 x 8 KB, two 22.5 KB halos, 8 KB
+// stencil, parameters).
 __host__ __device__ constexpr int ric_ctas_per_sm(ConvMode mode, int cout) {
     return mode == ConvMode::RicHalo && cout <= 64 ? 2 : 1;
 }
@@ -77,26 +69,28 @@ __host__ __device__ constexpr int ric_ctas_per_sm(ConvMode mode, int cout) {
 constexpr int kMaxRing = 8;
 __host__ __device__ constexpr int ring_cap(ConvMode mode) { return mode == ConvMode::Halo ? kMaxRing : kStages; }
 
+constexpr uint32_t kSmemMax = 227u * 1024u;      // dynamic shared memory per CTA (sm_90)
+
 // Shared memory from the 1024-aligned base: a ring of `stages` stages, then (RicHalo / Halo) two input-halo buffers and the
 // RicHalo stencil entries ([rotated tap m][tile pixel] x 8 B) or the Halo zero row (16 B, the A rows of K-padding slots), then
-// the epilogue parameters and (register A) the mbarriers.  The staged fp32 accumulators reuse everything before `par`.
+// the epilogue parameters and (conv_halo_kernel) the mbarriers.  The staged fp32 accumulators reuse everything before `par`.
 struct SmemLayout {
-    uint32_t stages;        // ring depth: kStages with A in shared memory; register A: as deep as 227 KB allows, <= ring_cap
-    uint32_t stage_bytes;   // A tile + B tile (register A: B tile only)
+    uint32_t stages;        // ring depth: kStages in conv_wgmma_kernel; conv_halo_kernel: as deep as 227 KB allows, <= ring_cap
+    uint32_t stage_bytes;   // A tile + B tile (conv_halo_kernel: B tile only)
     uint32_t halo;          // two input halos of halo_bytes each (halo_bytes = 0 in Tap / Ric mode)
     uint32_t halo_bytes;
     uint32_t aux;           // stencil (RicHalo) or zero row (Halo)
     uint32_t par;
-    uint32_t bars;          // register A: full[stages], empty[stages], halo full[2], halo empty[2] (8 B each)
+    uint32_t bars;          // conv_halo_kernel: full[stages], empty[stages], halo full[2], halo empty[2] (8 B each)
     uint32_t total;
 };
 
-__host__ __device__ inline SmemLayout smem_layout_at(ConvMode mode, int cout, int ksize, int up, int stages) {
+__host__ __device__ constexpr SmemLayout smem_layout_at(ConvMode mode, int cout, int ksize, int up, int stages) {
     const bool halo = mode == ConvMode::Halo, ric_halo = mode == ConvMode::RicHalo;
     const int rows = halo ? halo_rows(cout) : kTileH;
-    SmemLayout L;
+    SmemLayout L{};
     L.stages = static_cast<uint32_t>(stages);
-    L.stage_bytes = (register_a(mode, cout) ? 0u : static_cast<uint32_t>(kABytes)) + static_cast<uint32_t>(cout) * 128u;
+    L.stage_bytes = (uses_halo_kernel(mode) ? 0u : static_cast<uint32_t>(kABytes)) + static_cast<uint32_t>(cout) * 128u;
     L.halo = L.stages * L.stage_bytes;
     L.halo_bytes = halo       ? static_cast<uint32_t>((rows + ksize - 1) * (kTileW + ksize - 1)) * 128u
                    : ric_halo ? static_cast<uint32_t>(ric_halo_rows(up) * ric_halo_cols(up)) * 128u : 0u;
@@ -105,17 +99,28 @@ __host__ __device__ inline SmemLayout smem_layout_at(ConvMode mode, int cout, in
     const uint32_t staged = static_cast<uint32_t>(rows * kTileW) * acc_pitch(cout) * 4u;
     L.par = ((main_end > staged ? main_end : staged) + 15u) & ~15u;
     L.bars = L.par + par_bytes(cout);                    // a multiple of 8
-    L.total = L.bars + (register_a(mode, cout) ? (2 * L.stages + 4) * 8u : 0u);
+    L.total = L.bars + (uses_halo_kernel(mode) ? (2 * L.stages + 4) * 8u : 0u);
     return L;
 }
 
-__host__ __device__ inline SmemLayout smem_layout(ConvMode mode, int cout, int ksize, int up) {
-    if (!register_a(mode, cout)) return smem_layout_at(mode, cout, ksize, up, kStages);
+__host__ __device__ constexpr SmemLayout smem_layout(ConvMode mode, int cout, int ksize, int up) {
+    if (!uses_halo_kernel(mode)) return smem_layout_at(mode, cout, ksize, up, kStages);
     SmemLayout L = smem_layout_at(mode, cout, ksize, up, ring_cap(mode));
-    for (int s = ring_cap(mode) - 1; s >= kStages && L.total + 1024u > 227u * 1024u; --s)     // conv_smem_bytes <= 227 KB
+    for (int s = ring_cap(mode) - 1; s >= kStages && L.total + 1024u > kSmemMax; --s)     // conv_smem_bytes <= 227 KB
         L = smem_layout_at(mode, cout, ksize, up, s);
     return L;
 }
+
+// dynamic shared memory of a launch: the layout plus the slack for aligning the base to 1024 bytes
+constexpr size_t conv_smem_bytes(ConvMode mode, int cout, int ksize, int up) { return smem_layout(mode, cout, ksize, up).total + 1024; }
+
+// Every RicHalo launch fits: the widest piece of either precision at both source scales (up = 1: the fused nearest x2).
+// With no A ring, fp16 Cout 256 at up = 0 takes 189 KB (ring 4 x 32 KB, two 22.5 KB halos, stencil, parameters).
+static_assert(conv_smem_bytes(ConvMode::RicHalo, kMaxPiece(false), 3, 0) <= kSmemMax &&
+              conv_smem_bytes(ConvMode::RicHalo, kMaxPiece(false), 3, 1) <= kSmemMax &&
+              conv_smem_bytes(ConvMode::RicHalo, kMaxPiece(true), 3, 0) <= kSmemMax &&
+              conv_smem_bytes(ConvMode::RicHalo, kMaxPiece(true), 3, 1) <= kSmemMax,
+              "a RicHalo launch exceeds 227 KB of shared memory");
 
 __device__ __forceinline__ constexpr int ric_r0(int m) { return (m >= 2 && m <= 5) ? 0 : 1; }   // first corner row - 1 + 1
 __device__ __forceinline__ constexpr int ric_c0(int m) { return (m >= 4) ? 0 : 1; }
@@ -174,7 +179,7 @@ __device__ __forceinline__ float ric_blend(const RicWeightsF& w, float v00, floa
     return __fmaf_rn(w.w3, v11, __fmaf_rn(w.w2, v10, __fmaf_rn(w.w1, v01, __fmul_rn(w.w0, v00))));
 }
 
-// One A-row item of the shared-memory-A producers: the centre tap copies corner (0, 0); a rotated tap blends its corners
+// One A-row item of the gather producer: the centre tap copies corner (0, 0); a rotated tap blends its corners
 // with the stencil entry `entry()`.  `fetch(cy, cx, h)` returns 16 source bytes of corner (cy, cx), zeros outside the
 // (virtual, nearest-x2) image: the 8 fp16 channels (h = 0), or fp32 channels 4h .. 4h + 3.
 template <bool kExact, typename Entry, typename Fetch>
@@ -252,17 +257,10 @@ __device__ __forceinline__ void produce_ric(const ConvParams& p, int q, uint32_t
     }
 }
 
-// ---- RicHalo mode: what a CTA stages once, and the per-thread octants of its items (byte i = item row i)
-struct RicTile {
-    uint32_t halo, halo_bytes;  // two input-halo buffers: block b in buffer b & 1
-    uint32_t sten;              // stencil entries [m][pixel], 8 B each
-    uint32_t oct;
-};
-
 // The stencil entries of the tile's 128 pixels (fp16 weights or split-fp16 fractions: 8 B per rotated tap), stored
 // [m][pixel] so that the items of one load phase (neighbouring pixels, any sectors) hit distinct banks; zeros outside
-// Hout x Wout.  The octants go to registers: an item's output pixel never changes across chunks.  (They are read with
-// plain loads: a tile row of octant bytes is not 4-byte aligned when Wout is not a multiple of 4.)
+// Hout x Wout.  The octants go to registers (ric_lane): a lane's output pixels never change across chunks.  (They are read
+// with plain loads: a tile row of octant bytes is not 4-byte aligned when Wout is not a multiple of 4.)
 template <bool kExact>
 __device__ __forceinline__ void stage_ric_stencil(const ConvParams& p, uint32_t sten, int tid, int ty0, int tx0) {
     const uint8_t* table = kExact ? reinterpret_cast<const uint8_t*>(p.ric_lyx) : reinterpret_cast<const uint8_t*>(p.ric_wh);
@@ -279,16 +277,6 @@ __device__ __forceinline__ void stage_ric_stencil(const ConvParams& p, uint32_t 
 __device__ __forceinline__ uint32_t ric_oct(const ConvParams& p, int r, int ty0, int tx0) {
     const int oy = ty0 + (r >> 4), ox = tx0 + (r & 15);
     return (oy < p.Hout && ox < p.Wout) ? static_cast<uint32_t>(__ldg(p.ric_oct + static_cast<size_t>(oy) * p.Wout + ox)) : 0u;
-}
-
-template <bool kExact>
-__device__ __forceinline__ uint32_t load_ric_stencil(const ConvParams& p, uint32_t sten, int tid, int ty0, int tx0) {
-    using It = RicItems<kExact>;
-    stage_ric_stencil<kExact>(p, sten, tid, ty0, tx0);
-    uint32_t oct = 0;
-#pragma unroll
-    for (int i = 0; i < It::kRowsPer; ++i) oct |= ric_oct(p, tid / It::kSlots + It::kRowStep * i, ty0, tx0) << (8 * i);
-    return oct;
 }
 
 // The input of channel block `blk` for the whole tile: source rows (ty0 >> up) - 1 + [0, ric_halo_rows), columns
@@ -316,50 +304,10 @@ __device__ __forceinline__ void load_ric_halo(const ConvParams& p, int blk, uint
     }
 }
 
-// ---- RicHalo producer: the gather producer's items with the stencil entry from shared memory and the corners from the
-// block's halo.  A corner (vy, vx) of the virtual image is halo pixel ((vy >> up) - y0, (vx >> up) - x0); rows and columns past
-// Hout / Wout in ragged tiles stay inside the halo and produce zeros (`live`).  Bank conflicts: a load phase of 8 threads is
-// one pixel's 8 slots (fp16), or 2 horizontally adjacent pixels x 4 groups (split fp16) whose corners of one sector are
-// adjacent halo pixels, i.e. swizzle keys differing in bit 0: disjoint bank quads (2-way only where the two pixels' sectors
-// differ).  Stencil reads are broadcasts within a pixel and consecutive 8-byte words across pixels.
-template <bool kExact>
-__device__ __forceinline__ void produce_ric_halo(const ConvParams& p, int q, uint32_t a, int tid, int ty0, int tx0, const RicTile& rt) {
-    using It = RicItems<kExact>;
-    const int blk = q / 9, t = q - 9 * blk;
-    const int kq = t < 4 ? t : t - 1;
-    const int d = tid % It::kSlots, prow = tid / It::kSlots;
-    const bool valid = p.slots[blk * 8 + d].valid;
-    const uint32_t halo = rt.halo + static_cast<uint32_t>(blk & 1) * rt.halo_bytes;
-    const int hw = ric_halo_cols(p.up), y0 = (ty0 >> p.up) - 1, x0 = (tx0 >> p.up) - 1;
-#pragma unroll
-    for (int i = 0; i < It::kRowsPer; ++i) {
-        const int r = prow + It::kRowStep * i;
-        const int oy = ty0 + (r >> 4), ox = tx0 + (r & 15);
-        const bool live = valid && oy < p.Hout && ox < p.Wout;
-        int dy0 = 0, dx0 = 0, m = 0;
-        if (t != 4) {
-            m = (kq + (rt.oct >> (8 * i))) & 7;
-            dy0 = ric_r0(m) - 1; dx0 = ric_c0(m) - 1;
-        }
-        auto fetch = [&](int cy, int cx, int h) {
-            const int hp = (((oy + dy0 + cy) >> p.up) - y0) * hw + ((ox + dx0 + cx) >> p.up) - x0;
-            const uint32_t s = kExact ? static_cast<uint32_t>(2 * d + h) : static_cast<uint32_t>(d);
-            const uint4 v = ld_shared_v4(halo + static_cast<uint32_t>(hp) * 128u + ((s ^ static_cast<uint32_t>(hp & 7)) << 4));
-            return live ? v : make_uint4(0u, 0u, 0u, 0u);
-        };
-        auto entry = [&]() {
-            const uint2 raw = ld_shared_v2(rt.sten + static_cast<uint32_t>(m * kTileM + r) * 8u);
-            if constexpr (kExact) return make_float2(__uint_as_float(raw.x), __uint_as_float(raw.y));
-            else return raw;
-        };
-        ric_item<kExact>(t == 4, entry, fetch, a + static_cast<uint32_t>(r) * 128u, d, static_cast<uint32_t>(r & 7));
-    }
-}
-
-// ---- RicHalo mode with A in registers (Cout <= kRicRegMaxCout).  Lane l of warp w in warpgroup wg holds the A fragments
-// of tile pixels r = 64 wg + 16 w + l / 4 and r + 8 (fragment rows l / 4 and l / 4 + 8: tile row 4 wg + w, columns l / 4 and
-// l / 4 + 8), columns 2 (l % 4), +1 of the 16-byte slots 2k and 2k + 1 of K step k: the layout ldsm_x4 returns and mma_rs
-// takes, a[k][0 | 1] = slot 2k of pixel r | r + 8, a[k][2 | 3] = slot 2k + 1.  What a lane needs in every chunk:
+// ---- RicHalo mode, A in registers.  Lane l of warp w in warpgroup wg holds the A fragments of tile pixels
+// r = 64 wg + 16 w + l / 4 and r + 8 (fragment rows l / 4 and l / 4 + 8: tile row 4 wg + w, columns l / 4 and l / 4 + 8),
+// columns 2 (l % 4), +1 of the 16-byte slots 2k and 2k + 1 of K step k: the layout ldsm_x4 returns and mma_rs takes,
+// a[k][0 | 1] = slot 2k of pixel r | r + 8, a[k][2 | 3] = slot 2k + 1.  What a lane needs in every chunk:
 struct RicLane {
     int r;              // tile pixel of fragment row l / 4 (the other row is r + 8)
     int oy, ox;         // its output pixel (the other one is (oy, ox + 8))
@@ -386,8 +334,9 @@ __device__ __forceinline__ RicLane ric_lane(const ConvParams& p, int tid, int ty
 }
 
 // Chunk q's A fragments from the block's halo and the tile's stencil: the same corners, entries, blend helpers, centre
-// tap and zero rule as produce_ric_halo, so the fragments hold exactly the values that producer stores.  K-padding slots are
-// zeros in the halo and blend to zeros.
+// tap and zero rule as the gather producer (produce_ric), so the fragments hold exactly the values it stores.  A corner
+// (vy, vx) of the virtual image is halo pixel ((vy >> up) - y0, (vx >> up) - x0); pixels past Hout / Wout in ragged tiles
+// stay inside the halo and produce zeros (`live`).  K-padding slots are zeros in the halo and blend to zeros.
 //   fp16: per corner and K step one ldsm_x4 gathers the corner of each fragment row (every lane gives the row address of
 //   its ldmatrix pixel's corner), then each register is one packed-half2 blend with its row's weights.
 //   Split fp16: K steps 0-1 are the hi and 2-3 the lo parts of the chunk's 32 fp32 channels.  Channels 2t, 2t + 1 (t = l % 4)
@@ -485,19 +434,11 @@ __device__ __forceinline__ void produce_b(const ConvParams& p, int q, uint32_t d
     for (int i = tid; i < p.b_bytes / 16; i += kThreads) cp_async16(dst + 16u * i, src + 16 * i, 16u);
 }
 
-// chunk q: A rows and weight tile; in RicHalo mode the first chunk of block b also starts the halo of block b + 1
+// chunk q: A rows and weight tile
 template <ConvMode kMode, bool kExact>
-__device__ __forceinline__ void produce(const ConvParams& p, int q, uint32_t stage, int tid, int n, int ty0, int tx0, const RicTile& rt) {
-    if constexpr (kMode == ConvMode::Tap) {
-        produce_tap(p, q, stage, tid, n, ty0, tx0);
-    } else if constexpr (kMode == ConvMode::Ric) {
-        produce_ric<kExact>(p, q, stage, tid, n, ty0, tx0);
-    } else {
-        const int blk = q / 9;
-        if (q == 9 * blk && blk + 1 < p.nblocks)
-            load_ric_halo<kExact>(p, blk + 1, rt.halo + static_cast<uint32_t>((blk + 1) & 1) * rt.halo_bytes, tid, n, ty0, tx0);
-        produce_ric_halo<kExact>(p, q, stage, tid, ty0, tx0, rt);
-    }
+__device__ __forceinline__ void produce(const ConvParams& p, int q, uint32_t stage, int tid, int n, int ty0, int tx0) {
+    if constexpr (kMode == ConvMode::Tap) produce_tap(p, q, stage, tid, n, ty0, tx0);
+    else produce_ric<kExact>(p, q, stage, tid, n, ty0, tx0);
     produce_b(p, q, stage + kABytes, tid);
 }
 
@@ -618,19 +559,10 @@ __device__ __forceinline__ void store_tile(const ConvParams& p, uint8_t* smem, c
 
 // NC = Cout, PN = wgmma N per instruction (a divisor of NC: 32, 64 or 128).  Tap mode reads the split-fp16 K steps from
 // the K masks, so it is instantiated with kExact = false for both precisions.
-//
-// RicHalo mode here only for Cout > kRicRegMaxCout (narrower layers run conv_halo_kernel with A in registers): the
-// prologue stages the tile's stencil and the halo of channel block 0 (one cp.async group, waited for and
-// made visible by a barrier before chunk 0 is produced).  Producers run two chunks ahead: chunk c is produced in iteration
-// c - 2 (chunks 0 and 1 in the prologue), so the first chunk of block b (c = 9b) is produced in iteration 9b - 2, and the
-// halo of block b + 1 is issued there, in that iteration's cp.async group.  Block b + 1 is first read by chunk 9b + 9, produced
-// in iteration 9b + 7, whose cp_async_wait<kStages - 3> (every group but the newest, i.e. up to iteration 9b + 5's) and
-// barrier make it visible.  It overwrites the buffer of block b - 1, whose last chunk 9b - 1 was produced in iteration 9b - 3,
-// before the barrier of iteration 9b - 2.
 template <int NC, int PN, ConvMode kMode, bool kExact>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
-    static_assert(!register_a(kMode, NC), "conv_wgmma_kernel: shared-memory A modes only");
+    static_assert(!uses_halo_kernel(kMode), "conv_wgmma_kernel: Tap and Ric modes only");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_u32 = smem_u32(smem_raw);
     const uint32_t base = (raw_u32 + 1023u) & ~1023u;     // SWIZZLE_128B atoms are 1024-byte aligned
@@ -653,18 +585,10 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
 #pragma unroll
     for (int i = 0; i < NC / 2; ++i) acc[0][i] = 0.0f;
 
-    RicTile rt{base + L.halo, L.halo_bytes, base + L.aux, 0u};
-    if constexpr (kMode == ConvMode::RicHalo) {
-        rt.oct = load_ric_stencil<kExact>(p, rt.sten, tid, ty0, tx0);
-        load_ric_halo<kExact>(p, 0, rt.halo, tid, n, ty0, tx0);
-        cp_async_commit();
-        cp_async_wait<0>();
-        __syncthreads();                                  // stencil and halo 0 visible to every thread
-    }
     // prologue: chunks 0 and 1; every iteration commits one cp.async group so that "chunk q has landed" is wait_group 1
 #pragma unroll
     for (int s = 0; s < kStages - 2; ++s) {
-        if (s < nq) produce<kMode, kExact>(p, s, base + s * L.stage_bytes, tid, n, ty0, tx0, rt);
+        if (s < nq) produce<kMode, kExact>(p, s, base + s * L.stage_bytes, tid, n, ty0, tx0);
         cp_async_commit();
     }
     for (int q = 0; q < nq; ++q) {
@@ -678,7 +602,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
         mma_chunk<NC, PN>(acc[0], da, db, tail ? p.kmask_last : p.kmask_full, tail ? p.kmask2_last : p.kmask2_full);
         wgmma_commit();
         wgmma_wait<1>();                                  // this warpgroup's MMAs of chunk q - 1 have retired
-        if (q + kStages - 2 < nq) produce<kMode, kExact>(p, q + kStages - 2, base + ((q + kStages - 2) % kStages) * L.stage_bytes, tid, n, ty0, tx0, rt);
+        if (q + kStages - 2 < nq) produce<kMode, kExact>(p, q + kStages - 2, base + ((q + kStages - 2) % kStages) * L.stage_bytes, tid, n, ty0, tx0);
         cp_async_commit();
     }
     wgmma_wait<0>();
@@ -687,7 +611,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     store_tile<NC, 1>(p, smem, s_par, acc, tid, n, ty0, tx0);
 }
 
-// Halo and RicHalo (Cout <= kRicRegMaxCout) modes.  Chunk q belongs to channel block q / k^2 (every block but the last has
+// Halo and RicHalo modes.  Chunk q belongs to channel block q / k^2 (every block but the last has
 // exactly k^2 chunks, one per tap; in Halo mode the last one may pack several taps of its few channel groups into a chunk).
 // The mainloop is an mbarrier pipeline (below, and DESIGN section 4a): weight tiles in a ring of SmemLayout::stages
 // bulk-copied stages, halos with full / empty barriers per buffer, the halo of block b + 1 issued in the first iteration of
@@ -702,7 +626,7 @@ template <int NC, int PN, ConvMode kMode, bool kExact>
 __global__ void __launch_bounds__(kThreads, ric_ctas_per_sm(kMode, NC))
 conv_halo_kernel(const __grid_constant__ ConvParams p) {
     constexpr bool kRic = kMode == ConvMode::RicHalo;
-    static_assert(register_a(kMode, NC), "conv_halo_kernel: Halo, or RicHalo up to kRicRegMaxCout channels");
+    static_assert(uses_halo_kernel(kMode), "conv_halo_kernel: Halo and RicHalo modes only");
     constexpr int kRows = kRic ? kTileH : halo_rows(NC), kM = kRows * kTileW, MB = kM / 128;     // MB: m64 blocks per warpgroup
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_u32 = smem_u32(smem_raw);
@@ -852,21 +776,19 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
     store_tile<NC, MB>(p, smem, s_par, acc, tid, n, ty0, tx0);
 }
 
-size_t conv_smem_bytes(ConvMode mode, int cout, int ksize, int up) { return smem_layout(mode, cout, ksize, up).total + 1024; }
-
 namespace {
 
 template <ConvMode kMode, bool kExact, int NC, int PN>
 cudaError_t launch_one(const ConvParams& p, cudaStream_t stream) {
     constexpr int kRows = kMode == ConvMode::Halo ? halo_rows(NC) : kTileH;
     void (*kernel)(ConvParams);
-    if constexpr (register_a(kMode, NC)) kernel = conv_halo_kernel<NC, PN, kMode, kExact>;
+    if constexpr (uses_halo_kernel(kMode)) kernel = conv_halo_kernel<NC, PN, kMode, kExact>;
     else kernel = conv_wgmma_kernel<NC, PN, kMode, kExact>;
     static bool attr_set[64] = {};                        // the attribute is per function and context: one flag per device
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e == cudaSuccess && !(dev < 64 && attr_set[dev])) {
-        e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax);
         // two CTAs per SM need the largest shared-memory carveout of the unified L1 / shared-memory array
         if (e == cudaSuccess && ric_ctas_per_sm(kMode, NC) > 1)
             e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -902,7 +824,7 @@ cudaError_t launch_mode(const ConvParams& p, cudaStream_t stream) {
 }  // namespace
 
 cudaError_t launch_conv(const ConvParams& p, cudaStream_t stream) {
-    if (conv_smem_bytes(p.mode, p.Cout, p.ksize, p.up) > 227 * 1024 || p.b_bytes != p.Cout * 128) return cudaErrorInvalidConfiguration;
+    if (conv_smem_bytes(p.mode, p.Cout, p.ksize, p.up) > kSmemMax || p.b_bytes != p.Cout * 128) return cudaErrorInvalidConfiguration;
     switch (p.mode) {
         case ConvMode::Tap: return launch_mode<ConvMode::Tap, false>(p, stream);
         case ConvMode::Ric: return p.exact ? launch_mode<ConvMode::Ric, true>(p, stream) : launch_mode<ConvMode::Ric, false>(p, stream);

@@ -69,7 +69,6 @@ struct LayerDef {
     // compiled at finalize
     int first = 0;         // conv0-shaped: one <= 8-channel segment, stride 1, k > 3
     ConvMode mode = ConvMode::Tap;  // plan-time mode (Tap, Halo or Ric); conv_mode applies the run-time knobs
-    bool ric_halo_fits = false;     // the RicHalo shared-memory layout fits 227 KB
     int nchunks = 0, nblocks = 0;
     uint32_t kmask_full = 0xF, kmask_last = 0xF, kmask2_full = 0, kmask2_last = 0;
     Slot* d_slots = nullptr;
@@ -96,7 +95,7 @@ struct Knobs {
     int n128 = 1;             // Cout a multiple of 128: N = 128 wgmma instructions; 0 = N = 64 (two instructions per K step)
     int subpixel = 1;         // plan-time: stage-2 nearest-x2 + 3x3 as four 2x2 sub-pixel convolutions
     int derive_edge = 0;      // stage 2, no edge map passed: burn the edges pos2edge finds in the pos frames (fused into the ingest)
-    int ric_halo = 1;         // RIC layers whose shared-memory layout fits read stencil and corners from shared memory; 0 = gather
+    int ric_halo = 1;         // RIC layers read stencil and corners from shared memory (conv_halo_kernel); 0 = gather from global memory
 };
 struct KnobName { const char* name; int Knobs::*field; };
 const KnobName kKnobNames[] = {
@@ -435,10 +434,9 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     }
     L.first = (!L.ric && L.stride == 1 && L.up == 0 && L.sub < 0 && L.segs.size() == 1 && L.segs[0].nch <= 8 && k > 3 && L.pad == (k - 1) / 2) ? 1 : 0;
     // Halo mode needs k >= 2: the halo of block b + 1 is loaded in the first chunk of block b and read k^2 - 1 chunks later.
-    // The mode follows the layer's padded width, the same for every piece; whether RicHalo fits, the piece's width.
+    // The mode follows the layer's padded width, the same for every piece.
     L.mode = L.ric ? ConvMode::Ric
            : (L.stride == 1 && L.up == 0 && k >= 2 && (L.first || (E->knobs.halo && padded(C) <= 64))) ? ConvMode::Halo : ConvMode::Tap;
-    L.ric_halo_fits = L.ric && conv_smem_bytes(ConvMode::RicHalo, L.nw, k, L.up) <= 227 * 1024;
     L.nblocks = L.mode == ConvMode::Tap ? 0 : static_cast<int>(blocks.size());
     if (!L.ric) {
         std::vector<HSlot> all;
@@ -744,7 +742,7 @@ ActOut act_out(const dsu_engine* E, int buf, int choff) {
 // The mode a layer runs under the run-time knobs `first` and `ric_halo` (the rule: conv.cuh ConvMode)
 ConvMode conv_mode(const dsu_engine* E, const LayerDef& L) {
     if (L.mode == ConvMode::Halo && L.first && !E->knobs.first) return ConvMode::Tap;
-    if (L.mode == ConvMode::Ric && L.ric_halo_fits && E->knobs.ric_halo) return ConvMode::RicHalo;
+    if (L.mode == ConvMode::Ric && E->knobs.ric_halo) return ConvMode::RicHalo;
     return L.mode;
 }
 

@@ -346,8 +346,8 @@ class _Generator(nn.Module):
 
     def step_kernels(self):
         """``(name, kernel)`` of every launch of the current plan (C ABI ``dsu_step_kernel``: "halo", "tap", "ric_halo"
-        (stage-1 RIC with stencil and input staged in shared memory), "ric" (stage-1 RIC gathering from global memory), ...);
-        valid after the first forward."""
+        (stage-1 RIC with stencil and input staged in shared memory), "ric" (stage-1 RIC gathering from global memory,
+        knob ``ric_halo`` = 0), ...); valid after the first forward."""
         lib = capi.lib()
         out, i = [], 0
         while True:

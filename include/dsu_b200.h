@@ -132,7 +132,7 @@ int dsu_profile_forward(dsu_handle h, int32_t B, int32_t H, int32_t W, int32_t r
 const char* dsu_step_name(dsu_handle h, int32_t index);
 /* Mainloop launch i runs with the handle's current plan and knobs: "halo" (A fragments from a shared-memory input halo),
  * "tap" (A tiles gathered per tap), "ric_halo" (stage-1 deformable, stencil and corners from shared memory), "ric" (stage-1
- * deformable, gathered from global memory), or "maxpool" / "instance_norm" / "conv_12" for the other steps.  Valid after dsu_finalize. */
+ * deformable, gathered from global memory: knob "ric_halo" = 0), or "maxpool" / "instance_norm" / "conv_12" for the other steps.  Valid after dsu_finalize. */
 const char* dsu_step_kernel(dsu_handle h, int32_t index);
 
 /* ---- stand-alone uint8 / fp32 frame steps (device pointers) -------------------------------- */

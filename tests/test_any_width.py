@@ -94,6 +94,8 @@ for _stage in (1, 2):
         ("s%d-fp16-288-512-in" % _stage, _stage, "fp16",
          dict(filters=[40, 288, 512, 512, 288, 288], norm_layer="instance_norm", input_channels=5)),
     ]
+# fp16 stage 1: 480 = 256 + 224, both pieces of conv1, conv2 and the trunk without upsampling, the up-convolutions at 224
+LAYER_CONFIGS += [("s1-fp16-480-224", 1, "fp16", dict(filters=[32, 480, 480, 480, 224, 96]))]
 SHAPES = [(2, 20, 36), (1, 4, 4)]
 BUFS = {tl.SK0: 0, tl.P0: 0, tl.O1: 1, tl.P1: 1, tl.O2: 2, tl.TT: 2, tl.UU: 2, tl.V2: 4, tl.V1: 4, tl.C11: 5, tl.S0: 5,
         tl.RESID: 2}   # buffer -> index of the filters entry it stores
@@ -143,11 +145,10 @@ def _launch(name):
     return m.group(1), (int(m.group(2)) if m.group(2) else None), int(m.group(3) or 0)
 
 
-def _want_mode(stage, precision, args, layer, cls, nw):
-    """The mode rule of conv.cuh ConvMode at default knobs, from the layer's padded width and the piece width."""
+def _want_mode(stage, args, layer, cls):
+    """The mode rule of conv.cuh ConvMode at default knobs, from the layer's padded width."""
     if stage == 1:
-        fits = not (precision == "fp16" and nw >= 224 and not layer.startswith("upconv"))
-        return "ric_halo" if fits else "ric"
+        return "ric_halo"
     if layer == "conv0" and args["input_channels"] <= 8:
         return "halo"
     stride1 = layer not in ("conv1", "conv2") and not (layer.startswith("upconv") and cls is None)
@@ -170,7 +171,7 @@ def _check_launches(tag, m, sd, stage, precision, args, x, y, cache):
         npieces = -(-_pad(cout) // cap)
         assert (".n" in launch) == (npieces > 1), (tag, launch)
         c0, nw = piece * cap, min(cap, _pad(cout) - piece * cap)
-        assert mode == _want_mode(stage, precision, args, layer, cls, nw), (tag, launch, mode)
+        assert mode == _want_mode(stage, args, layer, cls), (tag, launch, mode)
         inputs, resid, outs, final = tl._io(stage, args, bufs, layer)
         if final:
             final_pieces = npieces

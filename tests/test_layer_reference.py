@@ -50,10 +50,12 @@ CONFIGS = [
     ("s2-16-c0-256", 2, "fp16", dict(filters=[256, 64, 64, 64, 64, 64]), {}),
     ("s1-16-a-c3", 1, "fp16", dict(filters=[32, 160, 192, 192, 224, 96], input_channels=3), {}),
     ("s1-16-b", 1, "fp16", dict(filters=[64, 96, 256, 256, 256, 128]), {}),
+    ("s1-16-c-224", 1, "fp16", dict(filters=[64, 224, 224, 224, 128, 224]), {}),
     ("s1-16-in", 1, "fp16", dict(filters=[32, 64, 128, 128, 128, 64], norm_layer="instance_norm", input_channels=1), {}),
 ]
 # Every kernel launch_mode (drawingspinup_b200/csrc/conv_wgmma.cu) instantiates: (mode, Cout, N piece, split fp16).  Tap
-# mode is instantiated once per (Cout, N) for both precisions; split fp16 stops at Cout 128.
+# mode is instantiated once per (Cout, N) for both precisions; split fp16 stops at Cout 128.  Tap and ric
+# entries name conv_wgmma_kernel instantiations; halo and ric_halo entries name conv_halo_kernel ones at every width.
 _PIECES = [(32, 32), (64, 64), (96, 32), (128, 128), (128, 64), (160, 32), (192, 64), (224, 32), (256, 128), (256, 64)]
 ALL_KERNELS = ({("tap", c, n, False) for c, n in _PIECES}
                | {(m, c, n, False) for m in ("ric", "ric_halo", "halo") for c, n in _PIECES}
@@ -219,8 +221,7 @@ def _check_forward(tag, m, sd, stage, precision, args, x, y, knobs, halo, cache,
         cout = _cout(args, layer)
         # which mode each launch must run (the rule: conv.cuh ConvMode)
         if stage == 1:
-            fits = not (precision == "fp16" and cout >= 224 and not layer.startswith("upconv"))
-            want = "ric_halo" if knobs["ric_halo"] and fits else "ric"
+            want = "ric_halo" if knobs["ric_halo"] else "ric"
         elif layer == "conv0" and cin <= 8:       # conv0-shaped: one 8-channel group
             want = "halo" if knobs["first"] else "tap"
         else:                                     # stride 1 without a fused nearest x2 (sub-pixel classes are stride 1)

@@ -5,8 +5,7 @@ With knob `ric_halo` = 1 a RIC launch stages its tile's stencil once per CTA and
 entry and corners from global memory per chunk.  Both feed the same corner values through the same blend into the same
 MMAs in the same order, so the stage-1 output and every intermediate buffer must be bit-identical, not merely close.
 Every comparison runs both settings on one handle and first checks from the plan (dsu_step_kernel) which producer each
-RIC launch ran.  Layers whose halo layout does not fit shared memory (fp16, Cout >= 224 without fused upsampling) keep
-the gather producer whatever the knob.
+RIC launch ran: with the knob on, every RIC launch at every width runs the halo producer.
 """
 import numpy as np
 import pytest
@@ -77,13 +76,12 @@ def _run_both(m, precision, args, x, dev):
     return out
 
 
-def _check(out, gather_layers=()):
-    """Knob 0: every RIC launch gathers.  Knob 1: every RIC launch but `gather_layers` (name prefixes) runs the halo
-    producer.  Output and every buffer bit-identical."""
+def _check(out):
+    """Knob 0: every RIC launch gathers.  Knob 1: every RIC launch runs the halo producer.  Output and every buffer
+    bit-identical."""
     (y0, k0, b0), (y1, k1, b1) = out[0], out[1]
     assert k0 and all(k == "ric" for k in k0.values()), k0
-    for n, k in k1.items():
-        assert k == ("ric" if any(n.startswith(p) for p in gather_layers) else "ric_halo"), (n, k)
+    assert k1.keys() == k0.keys() and all(k == "ric_halo" for k in k1.values()), k1
     assert torch.equal(y0, y1), (y1 - y0).abs().max().item()
     for buf in b0:
         assert torch.equal(b0[buf], b1[buf]), "buffer %d" % buf
@@ -135,14 +133,15 @@ def test_ric_halo_cout_96_and_n128(dev, monkeypatch, precision, n128):
     _check(_run_both(m, precision, args, x, dev))
 
 
-def test_ric_halo_fp16_wide_layers_fall_back(dev):
-    """fp16, filters[2..4] = 256: conv2 and the level-2 trunk (Cout 256, no fused upsampling, ~253 KB) do not fit the halo
-    layout and keep the gather producer; upconv2 / upconv1 (Cout 256 with the nearest x2, 6 x 10 halos, ~223 KB) and
-    conv_11 run the halo producer."""
-    args = dict(DEFAULT_ARGS, filters=[32, 64, 256, 256, 256, 64], resnet_blocks=2)
-    m, _ = _model(dev, "fp16", args, seed=9)
-    x = _frames(2, 40, 56, seed=23)
-    out = _run_both(m, "fp16", args, x, dev)
-    _check(out, gather_layers=("conv2", "resnets."))
-    kinds = out[1][1]
-    assert kinds["upconv2"] == kinds["upconv1"] == kinds["conv_11"] == "ric_halo"
+def test_ric_halo_fp16_wide_layers(dev, monkeypatch):
+    """fp16 launches wider than 128 channels, which only single-pass fp16 has: conv2 and the level-2 trunk at Cout 256 or
+    224 without upsampling (10 x 18 halos), the up-convolutions at 256 or 192 with the fused nearest x2 (6 x 10 halos),
+    conv1 at 160.  Cout 256 runs with N = 128 and N = 64 wgmma instructions."""
+    for filters, n128 in (([32, 64, 256, 256, 256, 64], "1"), ([32, 64, 256, 256, 256, 64], "0"),
+                          ([32, 160, 224, 224, 192, 96], "1")):
+        monkeypatch.setenv("DSU_N128", n128)
+        args = dict(DEFAULT_ARGS, filters=filters, resnet_blocks=2)
+        m, _ = _model(dev, "fp16", args, seed=9)
+        x = _frames(2, 40, 56, seed=23)
+        _check(_run_both(m, "fp16", args, x, dev))
+        del m

@@ -1,7 +1,7 @@
 """Per-launch device time of both stages (B=16, 512x512) through dsu_profile_forward (development aid).
-    python tools/layer_table.py [precision] [wide]
+    python tools/layer_table.py [precision] [wide | f0,f1,f2,f3,f4,f5]
 ``wide``: filters [64, 160, 288, 288, 192, 160], instance norm, no smoothers - layers in output-channel pieces and the split
-conv_12 step instead of the default configuration."""
+conv_12 step instead of the default configuration.  A comma-separated list: the default configuration with these filters."""
 import os
 import sys
 
@@ -16,6 +16,8 @@ prec = sys.argv[1] if len(sys.argv) > 1 else "fp16"
 args = dict(DEFAULT_ARGS)
 if len(sys.argv) > 2 and sys.argv[2] == "wide":
     args.update(filters=[64, 160, 288, 288, 192, 160], norm_layer="instance_norm", append_smoothers=False)
+elif len(sys.argv) > 2:
+    args.update(filters=[int(f) for f in sys.argv[2].split(",")])
 norm = args.get("norm_layer", "batch_norm")
 c, p, e = synth.make_frames(16, 512, 512, seed=1)
 c, p, e = torch.from_numpy(c).cuda(), torch.from_numpy(p).cuda(), torch.from_numpy(e).cuda()
