@@ -16,10 +16,11 @@ KIND_GENERATORJ_RIC = 1
 KIND_GENERATORJ = 2
 PREC_FP16 = 0
 PREC_FP16X3 = 1
+PREC_BF16 = 2
 NORM_NONE, NORM_BATCH, NORM_INSTANCE = 0, 1, 2
 E_NOTIMPL = -4
 
-PRECISIONS = {"fp16": PREC_FP16, "fp16x3": PREC_FP16X3}
+PRECISIONS = {"fp16": PREC_FP16, "fp16x3": PREC_FP16X3, "bf16": PREC_BF16}
 
 
 class DsuConfig(C.Structure):

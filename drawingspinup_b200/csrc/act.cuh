@@ -1,44 +1,60 @@
 // Activation storage: how a value that crosses a kernel boundary sits in HBM (NHWC, DESIGN section 3), and the device
-// helpers that convert and store it.  A buffer holds one of three forms, chosen per handle by engine.cu act_out:
+// helpers that convert and store it.  A buffer holds one of four forms, chosen per handle by engine.cu act_out:
 //   * fp16, one plane (fp16 mode);
+//   * bf16, one plane (bf16 mode): the same 2-byte elements, pitch and padding as the fp16 plane;
 //   * fp16 hi = fp16(v) and lo = fp16(v - hi), two planes (split-fp16 stage 2);
 //   * fp32 (split-fp16 stage 1: the RIC producers blend in fp32 and split after the blend).
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace dsu {
 
 // Where a kernel stores channel c of pixel p: element p * pitch + choff + c of `f32` when it is non-null, else of `hi`
-// (and of `lo` when non-null).  All null: no store.
+// (and of `lo` when non-null).  All null: no store.  `bf16`: the `hi` plane holds bf16 bits (never with a lo plane).
 struct ActOut {
     __half* hi;
     __half* lo;
     float* f32;
     int pitch, choff;
+    int bf16;
 };
 
+// Two fp32 <-> one 32-bit word of two 16-bit storage elements of type T (__half or __nv_bfloat16), round to nearest even
+template <typename T>
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
+    if constexpr (std::is_same<T, __nv_bfloat16>::value) {
+        __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+        return *reinterpret_cast<uint32_t*>(&h);
+    } else {
+        __half2 h = __floats2half2_rn(a, b);
+        return *reinterpret_cast<uint32_t*>(&h);
+    }
 }
+template <typename T>
 __device__ __forceinline__ float2 unpack_h2(uint32_t v) {
-    return __half22float2(*reinterpret_cast<const __half2*>(&v));
+    if constexpr (std::is_same<T, __nv_bfloat16>::value) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v));
+    else return __half22float2(*reinterpret_cast<const __half2*>(&v));
 }
+template <typename T>
 __device__ __forceinline__ void unpack8(const uint4& raw, float* f) {
-    float2 a = unpack_h2(raw.x), b = unpack_h2(raw.y), c = unpack_h2(raw.z), d = unpack_h2(raw.w);
+    float2 a = unpack_h2<T>(raw.x), b = unpack_h2<T>(raw.y), c = unpack_h2<T>(raw.z), d = unpack_h2<T>(raw.w);
     f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
 }
-// 8 fp32 -> packed fp16 (hi plane only)
+// 8 fp32 -> packed T (one plane)
+template <typename T>
 __device__ __forceinline__ uint4 pack8(const float* f) {
-    return make_uint4(pack_h2(f[0], f[1]), pack_h2(f[2], f[3]), pack_h2(f[4], f[5]), pack_h2(f[6], f[7]));
+    return make_uint4(pack_h2<T>(f[0], f[1]), pack_h2<T>(f[2], f[3]), pack_h2<T>(f[4], f[5]), pack_h2<T>(f[6], f[7]));
 }
 // 2 fp32 -> packed fp16 hi and residual lo = fp16(v - hi)
 __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-    hi = pack_h2(a, b);
-    const float2 r = unpack_h2(hi);
-    lo = pack_h2(a - r.x, b - r.y);
+    hi = pack_h2<__half>(a, b);
+    const float2 r = unpack_h2<__half>(hi);
+    lo = pack_h2<__half>(a - r.x, b - r.y);
 }
 // 8 fp32 -> packed fp16 hi and residual lo, two channels at a time
 __device__ __forceinline__ void split8(const float* f, uint4& hi, uint4& lo) {
@@ -74,9 +90,12 @@ __device__ __forceinline__ void store_act(const ActOut& o, size_t pix, int c, co
             for (int q = 0; q < N / 8; ++q) split8(f + 8 * q, h[q], l[q]);
 #pragma unroll
             for (int q = 0; q < N / 8; ++q) { reinterpret_cast<uint4*>(o.hi + i)[q] = h[q]; reinterpret_cast<uint4*>(o.lo + i)[q] = l[q]; }
+        } else if (o.bf16) {
+#pragma unroll
+            for (int q = 0; q < N / 8; ++q) reinterpret_cast<uint4*>(o.hi + i)[q] = pack8<__nv_bfloat16>(f + 8 * q);
         } else {
 #pragma unroll
-            for (int q = 0; q < N / 8; ++q) reinterpret_cast<uint4*>(o.hi + i)[q] = pack8(f + 8 * q);
+            for (int q = 0; q < N / 8; ++q) reinterpret_cast<uint4*>(o.hi + i)[q] = pack8<__half>(f + 8 * q);
         }
     }
 }

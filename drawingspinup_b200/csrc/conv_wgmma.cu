@@ -30,6 +30,10 @@
 // "Exact" mode (split fp16): a K chunk holds 32 channels as [a_hi | a_lo], its weight tile [W_hi | W_lo] in one
 // 128-byte row; A steps 0-3 are issued against B steps 0,1,0,1 and A steps 0,1 again against B steps 2,3 into the
 // same accumulator: a_hi*W_hi + a_lo*W_hi + a_hi*W_lo, fp32-grade products at 3x the tensor work.
+// Every kernel takes the element type T of its operands: __half (fp16, split fp16) or __nv_bfloat16 (bf16, single pass
+// like fp16, with the same chunks, tiles and launch shapes; only the wgmma type and the RIC blend differ).
+#include <type_traits>
+
 #include "conv_device.cuh"
 
 namespace dsu {
@@ -157,9 +161,15 @@ struct RicItems {
 // corner set of its sector in the operation order of the reference port of the weights: w00*n00, then fma w01*n01, w10*n10,
 // w11*n11.  fp16: the stencil entry holds the four fp16 weights {w00,w01 | w10,w11} and one call blends a packed-half2 word
 // (two channels).  Split fp16: the entry holds the fractions (ly, lx), the weights and the blend are fp32 with explicit
-// rounding, one channel per call.  Every RIC A producer goes through these two functions, so they all agree bit for bit.
+// rounding, one channel per call.  bf16: the split-fp16 entry and fp32 blend, one call per bf16 word (two channels), rounded
+// once to bf16 (a bf16 blend would round four partial sums at 2^-8 each).  The weight type selects the rule (RicWeightsH:
+// packed-half2; RicWeightsF: fp32), and every RIC A producer goes through these functions, so they all agree bit for bit.
 struct RicWeightsH { __half2 w00, w01, w10, w11; };
 struct RicWeightsF { float w0, w1, w2, w3; };
+
+// whether the RIC producers of a launch read the fp32 fractions (ric_lyx) and blend in fp32, not the fp16 weights (ric_wh)
+template <bool kExact, typename T>
+constexpr bool kBlendF32 = kExact || std::is_same<T, __nv_bfloat16>::value;
 
 __device__ __forceinline__ __half2 h2_of(uint32_t v) { return *reinterpret_cast<const __half2*>(&v); }
 
@@ -178,10 +188,16 @@ __device__ __forceinline__ uint32_t ric_blend(const RicWeightsH& w, uint32_t n00
 __device__ __forceinline__ float ric_blend(const RicWeightsF& w, float v00, float v01, float v10, float v11) {
     return __fmaf_rn(w.w3, v11, __fmaf_rn(w.w2, v10, __fmaf_rn(w.w1, v01, __fmul_rn(w.w0, v00))));
 }
+__device__ __forceinline__ uint32_t ric_blend(const RicWeightsF& w, uint32_t n00, uint32_t n01, uint32_t n10, uint32_t n11) {
+    const float2 a = unpack_h2<__nv_bfloat16>(n00), b = unpack_h2<__nv_bfloat16>(n01);
+    const float2 c = unpack_h2<__nv_bfloat16>(n10), d = unpack_h2<__nv_bfloat16>(n11);
+    return pack_h2<__nv_bfloat16>(ric_blend(w, a.x, b.x, c.x, d.x), ric_blend(w, a.y, b.y, c.y, d.y));
+}
 
 // One A-row item of the gather producer: the centre tap copies corner (0, 0); a rotated tap blends its corners
-// with the stencil entry `entry()`.  `fetch(cy, cx, h)` returns 16 source bytes of corner (cy, cx), zeros outside the
-// (virtual, nearest-x2) image: the 8 fp16 channels (h = 0), or fp32 channels 4h .. 4h + 3.
+// with the stencil entry `entry()` (fp16 weights or fp32 fractions: the blend rule above).  `fetch(cy, cx, h)` returns 16
+// source bytes of corner (cy, cx), zeros outside the (virtual, nearest-x2) image: the 8 fp16 / bf16 channels (h = 0), or
+// fp32 channels 4h .. 4h + 3.
 template <bool kExact, typename Entry, typename Fetch>
 __device__ __forceinline__ void ric_item(bool centre, const Entry& entry, const Fetch& fetch, uint32_t row, int d, uint32_t swz) {
     if constexpr (!kExact) {
@@ -189,7 +205,7 @@ __device__ __forceinline__ void ric_item(bool centre, const Entry& entry, const 
         if (centre) {
             out = fetch(0, 0, 0);
         } else {
-            const RicWeightsH w = ric_weights(entry());
+            const auto w = ric_weights(entry());
             const uint4 n00 = fetch(0, 0, 0), n01 = fetch(0, 1, 0), n10 = fetch(1, 0, 0), n11 = fetch(1, 1, 0);
             out = make_uint4(ric_blend(w, n00.x, n01.x, n10.x, n11.x), ric_blend(w, n00.y, n01.y, n10.y, n11.y),
                              ric_blend(w, n00.z, n01.z, n10.z, n11.z), ric_blend(w, n00.w, n01.w, n10.w, n11.w));
@@ -220,7 +236,7 @@ __device__ __forceinline__ void ric_item(bool centre, const Entry& entry, const 
 }
 
 // ---- RIC gather producer: octant, stencil entry and the four corners of every item straight from L2 / global memory
-template <bool kExact>
+template <bool kExact, typename T>
 __device__ __forceinline__ void produce_ric(const ConvParams& p, int q, uint32_t a, int tid, int n, int ty0, int tx0) {
     using It = RicItems<kExact>;
     const int blk = q / 9, t = q - 9 * blk;
@@ -250,20 +266,20 @@ __device__ __forceinline__ void produce_ric(const ConvParams& p, int q, uint32_t
             return ldg128_if(src + pix * pitch + 16 * h, ok);
         };
         auto entry = [&]() {
-            if constexpr (kExact) return live ? __ldg(p.ric_lyx + e * 8 + m) : make_float2(0.0f, 0.0f);
+            if constexpr (kBlendF32<kExact, T>) return live ? __ldg(p.ric_lyx + e * 8 + m) : make_float2(0.0f, 0.0f);
             else return live ? __ldg(p.ric_wh + e * 8 + m) : make_uint2(0u, 0u);
         };
         ric_item<kExact>(t == 4, entry, fetch, a + static_cast<uint32_t>(r) * 128u, d, static_cast<uint32_t>(r & 7));
     }
 }
 
-// The stencil entries of the tile's 128 pixels (fp16 weights or split-fp16 fractions: 8 B per rotated tap), stored
+// The stencil entries of the tile's 128 pixels (fp16 weights or, kF32, fp32 fractions: 8 B per rotated tap), stored
 // [m][pixel] so that the items of one load phase (neighbouring pixels, any sectors) hit distinct banks; zeros outside
 // Hout x Wout.  The octants go to registers (ric_lane): a lane's output pixels never change across chunks.  (They are read
 // with plain loads: a tile row of octant bytes is not 4-byte aligned when Wout is not a multiple of 4.)
-template <bool kExact>
+template <bool kF32>
 __device__ __forceinline__ void stage_ric_stencil(const ConvParams& p, uint32_t sten, int tid, int ty0, int tx0) {
-    const uint8_t* table = kExact ? reinterpret_cast<const uint8_t*>(p.ric_lyx) : reinterpret_cast<const uint8_t*>(p.ric_wh);
+    const uint8_t* table = kF32 ? reinterpret_cast<const uint8_t*>(p.ric_lyx) : reinterpret_cast<const uint8_t*>(p.ric_wh);
     for (int i = tid; i < kTileM * 8; i += kThreads) {
         const int r = i >> 3, m = i & 7;
         const int oy = ty0 + (r >> 4), ox = tx0 + (r & 15);
@@ -337,12 +353,13 @@ __device__ __forceinline__ RicLane ric_lane(const ConvParams& p, int tid, int ty
 // tap and zero rule as the gather producer (produce_ric), so the fragments hold exactly the values it stores.  A corner
 // (vy, vx) of the virtual image is halo pixel ((vy >> up) - y0, (vx >> up) - x0); pixels past Hout / Wout in ragged tiles
 // stay inside the halo and produce zeros (`live`).  K-padding slots are zeros in the halo and blend to zeros.
-//   fp16: per corner and K step one ldsm_x4 gathers the corner of each fragment row (every lane gives the row address of
-//   its ldmatrix pixel's corner), then each register is one packed-half2 blend with its row's weights.
+//   fp16 / bf16: per corner and K step one ldsm_x4 gathers the corner of each fragment row (every lane gives the row address
+//   of its ldmatrix pixel's corner), then each register is one blend of two channels with its row's weights (packed-half2
+//   in fp16, fp32 and one rounding in bf16).
 //   Split fp16: K steps 0-1 are the hi and 2-3 the lo parts of the chunk's 32 fp32 channels.  Channels 2t, 2t + 1 (t = l % 4)
 //   of group g sit in halo slot 2g + (t >> 1) at byte 8 (t & 1): one ld.shared.v2 per corner, group and pixel; the blend is
 //   split once, hi into K step g / 2 and lo into g / 2 + 2.
-template <bool kExact>
+template <bool kExact, typename T>
 __device__ __forceinline__ void build_ric_a(const ConvParams& p, int q, uint32_t halo, uint32_t sten, const RicLane& ln,
                                             int lane, int ty0, int tx0, uint32_t (*a)[4]) {
     const int t = q % 9, kq = t < 4 ? t : t - 1;
@@ -364,9 +381,13 @@ __device__ __forceinline__ void build_ric_a(const ConvParams& p, int q, uint32_t
             sector(2, dy0, dx0);
             const int vy = ln.oy + dy0, vx = ln.ax + dx0;
             const int h00 = hpix(vy, vx), h01 = hpix(vy, vx + 1), h10 = hpix(vy + 1, vx), h11 = hpix(vy + 1, vx + 1);
-            RicWeightsH w[2];
+            auto weights = [](uint2 raw) {        // the staged entry: fp32 fractions (bf16) or fp16 weights
+                if constexpr (kBlendF32<kExact, T>) return ric_weights(make_float2(__uint_as_float(raw.x), __uint_as_float(raw.y)));
+                else return ric_weights(raw);
+            };
+            decltype(weights(uint2{})) w[2];
 #pragma unroll
-            for (int j = 0; j < 2; ++j) w[j] = ric_weights(ld_shared_v2(sten + static_cast<uint32_t>(sector(j, dy0, dx0) * kTileM + ln.r + 8 * j) * 8u));
+            for (int j = 0; j < 2; ++j) w[j] = weights(ld_shared_v2(sten + static_cast<uint32_t>(sector(j, dy0, dx0) * kTileM + ln.r + 8 * j) * 8u));
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 uint32_t n00[4], n01[4], n10[4], n11[4];
@@ -435,20 +456,20 @@ __device__ __forceinline__ void produce_b(const ConvParams& p, int q, uint32_t d
 }
 
 // chunk q: A rows and weight tile
-template <ConvMode kMode, bool kExact>
+template <ConvMode kMode, bool kExact, typename T>
 __device__ __forceinline__ void produce(const ConvParams& p, int q, uint32_t stage, int tid, int n, int ty0, int tx0) {
     if constexpr (kMode == ConvMode::Tap) produce_tap(p, q, stage, tid, n, ty0, tx0);
-    else produce_ric<kExact>(p, q, stage, tid, n, ty0, tx0);
+    else produce_ric<kExact, T>(p, q, stage, tid, n, ty0, tx0);
     produce_b(p, q, stage + kABytes, tid);
 }
 
 // the K steps of one chunk: every PN-column piece of the accumulator against the matching PN rows of the weight tile
-template <int NC, int PN>
+template <int NC, int PN, typename T>
 __device__ __forceinline__ void mma_chunk(float* acc, uint64_t da, uint64_t db, uint32_t km, uint32_t km2) {
     constexpr uint64_t kPieceStep = PN * 128 / 16;        // descriptor units between PN-row weight pieces
     auto step = [&](int ka, int kb) {
 #pragma unroll
-        for (int j = 0; j < NC / PN; ++j) Wgmma<PN>::mma(acc + j * (PN / 2), da + 2 * ka, db + 2 * kb + j * kPieceStep);
+        for (int j = 0; j < NC / PN; ++j) Wgmma<PN, T>::mma(acc + j * (PN / 2), da + 2 * ka, db + 2 * kb + j * kPieceStep);
     };
     if (km2) {
         // split-fp16: A = [a_hi | a_lo] (steps 0-1 | 2-3), B = [W_hi | W_lo]; a_hi*W_hi + a_lo*W_hi + a_hi*W_lo
@@ -468,14 +489,14 @@ __device__ __forceinline__ void mma_chunk(float* acc, uint64_t da, uint64_t db, 
 // the same K steps with A from registers: a[mb][k] = K step k of m64 block mb; in split-fp16 the hi fragments (steps 0-1)
 // are used for both a_hi*W_hi and a_hi*W_lo.  Every step is issued, also in the ragged last chunk: its K-padding slots
 // read zeros against zero weights and add exact zeros, and a branch-free sequence keeps the wgmmas back to back.
-template <int NC, int PN, int MB, bool kExact>
+template <int NC, int PN, int MB, bool kExact, typename T>
 __device__ __forceinline__ void mma_chunk_rs(float (*acc)[NC / 2], const uint32_t (*a)[4][4], uint64_t db) {
     constexpr uint64_t kPieceStep = PN * 128 / 16;
     auto step = [&](int ka, int kb) {
 #pragma unroll
         for (int mb = 0; mb < MB; ++mb)
 #pragma unroll
-            for (int j = 0; j < NC / PN; ++j) Wgmma<PN>::mma_rs(acc[mb] + j * (PN / 2), a[mb][ka], db + 2 * kb + j * kPieceStep);
+            for (int j = 0; j < NC / PN; ++j) Wgmma<PN, T>::mma_rs(acc[mb] + j * (PN / 2), a[mb][ka], db + 2 * kb + j * kPieceStep);
     };
 #pragma unroll
     for (int k = 0; k < 4; ++k) step(k, kExact ? (k & 1) : k);
@@ -557,9 +578,9 @@ __device__ __forceinline__ void store_tile(const ConvParams& p, uint8_t* smem, c
 
 }  // namespace
 
-// NC = Cout, PN = wgmma N per instruction (a divisor of NC: 32, 64 or 128).  Tap mode reads the split-fp16 K steps from
-// the K masks, so it is instantiated with kExact = false for both precisions.
-template <int NC, int PN, ConvMode kMode, bool kExact>
+// NC = Cout, PN = wgmma N per instruction (a divisor of NC: 32, 64 or 128), T the operand type.  Tap mode reads the
+// split-fp16 K steps from the K masks, so it is instantiated with kExact = false for both fp16 precisions.
+template <int NC, int PN, ConvMode kMode, bool kExact, typename T>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     static_assert(!uses_halo_kernel(kMode), "conv_wgmma_kernel: Tap and Ric modes only");
@@ -588,7 +609,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
     // prologue: chunks 0 and 1; every iteration commits one cp.async group so that "chunk q has landed" is wait_group 1
 #pragma unroll
     for (int s = 0; s < kStages - 2; ++s) {
-        if (s < nq) produce<kMode, kExact>(p, s, base + s * L.stage_bytes, tid, n, ty0, tx0);
+        if (s < nq) produce<kMode, kExact, T>(p, s, base + s * L.stage_bytes, tid, n, ty0, tx0);
         cp_async_commit();
     }
     for (int q = 0; q < nq; ++q) {
@@ -599,10 +620,10 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
         const uint64_t da = wgmma_desc_sw128(stage + wg * (kABytes / 2), 1024), db = wgmma_desc_sw128(stage + kABytes, 1024);
         const bool tail = q >= tail_from;
         wgmma_fence();
-        mma_chunk<NC, PN>(acc[0], da, db, tail ? p.kmask_last : p.kmask_full, tail ? p.kmask2_last : p.kmask2_full);
+        mma_chunk<NC, PN, T>(acc[0], da, db, tail ? p.kmask_last : p.kmask_full, tail ? p.kmask2_last : p.kmask2_full);
         wgmma_commit();
         wgmma_wait<1>();                                  // this warpgroup's MMAs of chunk q - 1 have retired
-        if (q + kStages - 2 < nq) produce<kMode, kExact>(p, q + kStages - 2, base + ((q + kStages - 2) % kStages) * L.stage_bytes, tid, n, ty0, tx0);
+        if (q + kStages - 2 < nq) produce<kMode, kExact, T>(p, q + kStages - 2, base + ((q + kStages - 2) % kStages) * L.stage_bytes, tid, n, ty0, tx0);
         cp_async_commit();
     }
     wgmma_wait<0>();
@@ -622,7 +643,7 @@ conv_wgmma_kernel(const __grid_constant__ ConvParams p) {
 // the prologue (build_ric_a), with 8 x 16 tiles and k^2 = 9 taps per block.  RicHalo layers up to 64 channels run two
 // CTAs per SM (ric_ctas_per_sm) with one fragment buffer, so one CTA's fragment building and barriers overlap the other's
 // MMAs.
-template <int NC, int PN, ConvMode kMode, bool kExact>
+template <int NC, int PN, ConvMode kMode, bool kExact, typename T>
 __global__ void __launch_bounds__(kThreads, ric_ctas_per_sm(kMode, NC))
 conv_halo_kernel(const __grid_constant__ ConvParams p) {
     constexpr bool kRic = kMode == ConvMode::RicHalo;
@@ -697,7 +718,7 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
         cp_async_mbar_arrive(hfull_bar(blk));
     };
     auto load_frags = [&](int q, int b, uint32_t (*dst)[4][4]) {      // chunk q of channel block b
-        if constexpr (kRic) build_ric_a<kExact>(p, q, halo_buf(b), aux, ln, lane, ty0, tx0, dst[0]);
+        if constexpr (kRic) build_ric_a<kExact, T>(p, q, halo_buf(b), aux, ln, lane, ty0, tx0, dst[0]);
         else load_a<MB>(p, q, halo_buf(b), aux, pb, lane, dst);
     };
     // thread 0: weight tile of chunk c (one bulk copy) into stage s
@@ -708,7 +729,7 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
     };
 
     // prologue: (RicHalo: the tile's stencil with) the halo of block 0, and the weight tiles of chunks 0 .. S - 3
-    if constexpr (kRic) stage_ric_stencil<kExact>(p, aux, tid, ty0, tx0);
+    if constexpr (kRic) stage_ric_stencil<kBlendF32<kExact, T>>(p, aux, tid, ty0, tx0);
     load_block(0);
     if (tid == 0)
         for (int c = 0; c < S - 2 && c < nq; ++c) produce_w(c, c);
@@ -729,7 +750,7 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
         mbar_wait(full_bar(qs), qph);
         const uint64_t db = wgmma_desc_sw128(base + static_cast<uint32_t>(qs) * L.stage_bytes, 1024);
         wgmma_fence();
-        mma_chunk_rs<NC, PN, MB, kExact>(acc, cur, db);
+        mma_chunk_rs<NC, PN, MB, kExact, T>(acc, cur, db);
         wgmma_commit();
         if constexpr (kOneBuf) {
             wgmma_wait<0>();                              // the MMAs of chunk q have retired: the one buffer is free
@@ -778,12 +799,12 @@ conv_halo_kernel(const __grid_constant__ ConvParams p) {
 
 namespace {
 
-template <ConvMode kMode, bool kExact, int NC, int PN>
+template <ConvMode kMode, bool kExact, typename T, int NC, int PN>
 cudaError_t launch_one(const ConvParams& p, cudaStream_t stream) {
     constexpr int kRows = kMode == ConvMode::Halo ? halo_rows(NC) : kTileH;
     void (*kernel)(ConvParams);
-    if constexpr (uses_halo_kernel(kMode)) kernel = conv_halo_kernel<NC, PN, kMode, kExact>;
-    else kernel = conv_wgmma_kernel<NC, PN, kMode, kExact>;
+    if constexpr (uses_halo_kernel(kMode)) kernel = conv_halo_kernel<NC, PN, kMode, kExact, T>;
+    else kernel = conv_wgmma_kernel<NC, PN, kMode, kExact, T>;
     static bool attr_set[64] = {};                        // the attribute is per function and context: one flag per device
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
@@ -800,37 +821,45 @@ cudaError_t launch_one(const ConvParams& p, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
-template <ConvMode kMode, bool kExact>
+template <ConvMode kMode, bool kExact, typename T>
 cudaError_t launch_mode(const ConvParams& p, cudaStream_t stream) {
     switch (p.Cout) {
-        case 32: return launch_one<kMode, kExact, 32, 32>(p, stream);
-        case 64: return launch_one<kMode, kExact, 64, 64>(p, stream);
-        case 96: return launch_one<kMode, kExact, 96, 32>(p, stream);
-        case 128: return p.n128 ? launch_one<kMode, kExact, 128, 128>(p, stream) : launch_one<kMode, kExact, 128, 64>(p, stream);
+        case 32: return launch_one<kMode, kExact, T, 32, 32>(p, stream);
+        case 64: return launch_one<kMode, kExact, T, 64, 64>(p, stream);
+        case 96: return launch_one<kMode, kExact, T, 96, 32>(p, stream);
+        case 128: return p.n128 ? launch_one<kMode, kExact, T, 128, 128>(p, stream) : launch_one<kMode, kExact, T, 128, 64>(p, stream);
         default: break;
     }
     if constexpr (!kExact) {              // split-fp16 launches stop at 128 channels (wider layers run in pieces, conv.cuh kMaxPiece)
         switch (p.Cout) {
-            case 160: return launch_one<kMode, kExact, 160, 32>(p, stream);
-            case 192: return launch_one<kMode, kExact, 192, 64>(p, stream);
-            case 224: return launch_one<kMode, kExact, 224, 32>(p, stream);
-            case 256: return p.n128 ? launch_one<kMode, kExact, 256, 128>(p, stream) : launch_one<kMode, kExact, 256, 64>(p, stream);
+            case 160: return launch_one<kMode, kExact, T, 160, 32>(p, stream);
+            case 192: return launch_one<kMode, kExact, T, 192, 64>(p, stream);
+            case 224: return launch_one<kMode, kExact, T, 224, 32>(p, stream);
+            case 256: return p.n128 ? launch_one<kMode, kExact, T, 256, 128>(p, stream) : launch_one<kMode, kExact, T, 256, 64>(p, stream);
             default: break;
         }
     }
     return cudaErrorInvalidConfiguration;
 }
 
+// the launch's precision: split fp16 (Tap mode reads it from the K masks), fp16 or bf16
+template <ConvMode kMode>
+cudaError_t launch_prec(const ConvParams& p, cudaStream_t stream) {
+    if constexpr (kMode != ConvMode::Tap)
+        if (p.exact) return launch_mode<kMode, true, __half>(p, stream);
+    return p.bf16 ? launch_mode<kMode, false, __nv_bfloat16>(p, stream) : launch_mode<kMode, false, __half>(p, stream);
+}
+
 }  // namespace
 
 cudaError_t launch_conv(const ConvParams& p, cudaStream_t stream) {
-    if (conv_smem_bytes(p.mode, p.Cout, p.ksize, p.up) > kSmemMax || p.b_bytes != p.Cout * 128) return cudaErrorInvalidConfiguration;
+    if (conv_smem_bytes(p.mode, p.Cout, p.ksize, p.up) > kSmemMax || p.b_bytes != p.Cout * 128 || (p.exact && p.bf16))
+        return cudaErrorInvalidConfiguration;
     switch (p.mode) {
-        case ConvMode::Tap: return launch_mode<ConvMode::Tap, false>(p, stream);
-        case ConvMode::Ric: return p.exact ? launch_mode<ConvMode::Ric, true>(p, stream) : launch_mode<ConvMode::Ric, false>(p, stream);
-        case ConvMode::RicHalo:
-            return p.exact ? launch_mode<ConvMode::RicHalo, true>(p, stream) : launch_mode<ConvMode::RicHalo, false>(p, stream);
-        case ConvMode::Halo: return p.exact ? launch_mode<ConvMode::Halo, true>(p, stream) : launch_mode<ConvMode::Halo, false>(p, stream);
+        case ConvMode::Tap: return launch_prec<ConvMode::Tap>(p, stream);
+        case ConvMode::Ric: return launch_prec<ConvMode::Ric>(p, stream);
+        case ConvMode::RicHalo: return launch_prec<ConvMode::RicHalo>(p, stream);
+        case ConvMode::Halo: return launch_prec<ConvMode::Halo>(p, stream);
     }
     return cudaErrorInvalidConfiguration;
 }

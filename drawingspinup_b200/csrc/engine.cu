@@ -3,9 +3,10 @@
 // Turns the constructor arguments of GeneratorJ / GeneratorJ_RIC (training/models.py:24-111,
 // 200-291) and a loaded state dict into a list of fused convolution launches (conv_wgmma.cu):
 // BatchNorm (eval) is folded into per-channel scale/shift, conv weights are rounded to fp16
-// (hi [+lo]) and pre-swizzled into tensor-core tiles, skip connections / nearest-x2 upsampling /
+// (hi [+lo]) or bf16 and pre-swizzled into tensor-core tiles, skip connections / nearest-x2 upsampling /
 // stride / concat become slot tables, and the dead stage-1 smoother conv (models.py:348-350) is
 // dropped.  Activations live in NHWC workspace buffers owned by the handle, in one of the forms of act.cuh.
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -142,6 +143,7 @@ struct dsu_engine {
     Knobs knobs;
     int cin_pad = 8;
     bool exact = false, finalized = false;
+    bool bf16 = false;        // DSU_PREC_BF16: bf16 weights and activation planes (single pass, the fp16 plan)
     std::map<std::string, std::vector<int64_t>> expected;
     std::vector<std::string> expected_order;
     std::map<std::string, std::vector<float>> w;
@@ -478,7 +480,8 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
     const size_t tile = static_cast<size_t>(L.nw) * 128;   // the piece's output channels; rows past cout stay zero
     std::vector<uint8_t> pack(static_cast<size_t>(L.nchunks) * tile, 0);
     size_t off = 0;
-    auto put = [&](size_t tile_off, int row, int slot, int ci, __half val) {
+    auto put = [&](size_t tile_off, int row, int slot, int ci, auto val) {     // val: __half or __nv_bfloat16
+        static_assert(sizeof(val) == 2, "16-bit weight elements");
         const size_t b = tile_off + static_cast<size_t>(row) * 128 + ((static_cast<size_t>(slot) ^ (row & 7)) << 4) + ci * 2;
         std::memcpy(&pack[b], &val, 2);
     };
@@ -491,6 +494,10 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
                 const HSlot& h = ds[d];
                 for (int ci = 0; ci < h.nvalid; ++ci) {
                     const float wv = Wt[((static_cast<size_t>(L.n0 + o) * cin_total + h.wch + ci) * k + h.kh) * k + h.kw];
+                    if (E->bf16) {
+                        put(off, o, d, ci, __float2bfloat16_rn(wv));
+                        continue;
+                    }
                     const __half wh = __float2half_rn(wv);
                     put(off, o, d, ci, wh);
                     if (exact) put(off, o, d + 4, ci, __float2half_rn(wv - __half2float(wh)));   // [W_hi | W_lo] in one row
@@ -736,7 +743,7 @@ int ensure_shape(dsu_engine* E, int B, int H, int W) {
 ActOut act_out(const dsu_engine* E, int buf, int choff) {
     if (buf < 0) return ActOut{};
     if (E->f32_acts) return ActOut{nullptr, nullptr, reinterpret_cast<float*>(E->buf_hi[buf]), E->buf_C[buf], choff};
-    return ActOut{E->buf_hi[buf], E->buf_lo[buf], nullptr, E->buf_C[buf], choff};
+    return ActOut{E->buf_hi[buf], E->buf_lo[buf], nullptr, E->buf_C[buf], choff, E->bf16 ? 1 : 0};
 }
 
 // The mode a layer runs under the run-time knobs `first` and `ric_halo` (the rule: conv.cuh ConvMode)
@@ -780,7 +787,7 @@ int run_network(dsu_engine* E, int B, int H, int W, float* y_dev, uint8_t* y_rgb
         const int src_level = E->buf_level[L.segs[0].buf];
         p.Hin = H >> src_level; p.Win = W >> src_level;
         p.up = L.up; p.Hv = p.Hin << L.up; p.Wv = p.Win << L.up;
-        p.mode = conv_mode(E, L); p.stride = L.stride; p.exact = E->exact ? 1 : 0;
+        p.mode = conv_mode(E, L); p.stride = L.stride; p.exact = E->exact ? 1 : 0; p.bf16 = E->bf16 ? 1 : 0;
         p.nchunks = L.nchunks; p.nblocks = L.nblocks; p.Cout = L.nw;
         p.b_bytes = L.nw * 128;
         p.kmask_full = L.kmask_full; p.kmask_last = L.kmask_last; p.kmask2_full = L.kmask2_full; p.kmask2_last = L.kmask2_last;
@@ -867,7 +874,8 @@ int dsu_create(const dsu_config* cfg, dsu_handle* out) {
     if (cfg->kind != DSU_KIND_GENERATORJ_RIC && cfg->kind != DSU_KIND_GENERATORJ)
         return fail(DSU_E_INVALID, "kind must be DSU_KIND_GENERATORJ_RIC or DSU_KIND_GENERATORJ");
     if (cfg->norm != DSU_NORM_BATCH && cfg->norm != DSU_NORM_NONE && cfg->norm != DSU_NORM_INSTANCE) return fail(DSU_E_INVALID, "bad norm");
-    if (cfg->precision != DSU_PREC_FP16 && cfg->precision != DSU_PREC_FP16X3) return fail(DSU_E_INVALID, "bad precision");
+    if (cfg->precision != DSU_PREC_FP16 && cfg->precision != DSU_PREC_FP16X3 && cfg->precision != DSU_PREC_BF16)
+        return fail(DSU_E_INVALID, "bad precision");
     if (cfg->input_channels < 1 || cfg->input_channels > 16) return fail(DSU_E_INVALID, "input_channels must be in [1,16]");
     if (cfg->resnet_blocks < 0 || cfg->resnet_blocks > 64) return fail(DSU_E_INVALID, "resnet_blocks out of range");
     for (int i = 0; i < 6; ++i)
@@ -888,6 +896,7 @@ int dsu_create(const dsu_config* cfg, dsu_handle* out) {
     E->knobs = knobs_from_env();
     E->cin_pad = (cfg->input_channels + 7) / 8 * 8;
     E->exact = cfg->precision == DSU_PREC_FP16X3;
+    E->bf16 = cfg->precision == DSU_PREC_BF16;
     E->f32_acts = cfg->kind == DSU_KIND_GENERATORJ_RIC && E->exact;
     int rc = build_plan(E);
     if (rc) { delete E; return rc; }

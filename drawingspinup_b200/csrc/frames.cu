@@ -42,7 +42,8 @@ __global__ void frames_to_tensor_kernel(const uchar4* __restrict__ color, const 
     if (mask_out) mask_out[p] = mask;
 }
 
-// 2x2 / stride 2 max-pool over NHWC fp16 (8 channels per thread)
+// 2x2 / stride 2 max-pool over one NHWC plane of 16-bit elements T, fp16 or bf16 (8 channels per thread)
+template <typename T>
 __global__ void maxpool2_kernel(const __half* __restrict__ in, int in_pitch, int B, int Hin, int Win, int C, __half* out, int out_pitch) {
     const int Ho = Hin / 2, Wo = Win / 2, G = C / 8;
     const size_t total = static_cast<size_t>(B) * Ho * Wo * G;
@@ -58,12 +59,12 @@ __global__ void maxpool2_kernel(const __half* __restrict__ in, int in_pitch, int
     for (int k = 0; k < 4; ++k) {
         const size_t ip = (static_cast<size_t>(n) * Hin + 2 * oy + (k >> 1)) * Win + 2 * ox + (k & 1);
         float v[8];
-        unpack8(*reinterpret_cast<const uint4*>(in + ip * in_pitch + g * 8), v);
+        unpack8<T>(*reinterpret_cast<const uint4*>(in + ip * in_pitch + g * 8), v);
 #pragma unroll
         for (int c = 0; c < 8; ++c)      // strict > keeps the first maximum, like F.max_pool2d's value
             if (k == 0 || v[c] > best[c]) best[c] = v[c];
     }
-    *reinterpret_cast<uint4*>(out + op * out_pitch + g * 8) = pack8(best);
+    *reinterpret_cast<uint4*>(out + op * out_pitch + g * 8) = pack8<T>(best);
 }
 
 // the same pool over fp32 NHWC (4 channels per thread)
@@ -84,7 +85,7 @@ __global__ void maxpool2_f32_kernel(const float* __restrict__ in, int in_pitch, 
         const size_t ip = (static_cast<size_t>(n) * Hin + 2 * oy + (k >> 1)) * Win + 2 * ox + (k & 1);
         const float4 v = *reinterpret_cast<const float4*>(in + ip * in_pitch + g * 4);
         if (k == 0) best = v;
-        else {      // strict > keeps the first maximum, like the fp16 kernel above and F.max_pool2d's value
+        else {      // strict > keeps the first maximum, like the 16-bit kernel above and F.max_pool2d's value
             if (v.x > best.x) best.x = v.x;
             if (v.y > best.y) best.y = v.y;
             if (v.z > best.z) best.z = v.z;
@@ -293,14 +294,14 @@ cudaError_t frames_to_tensor(const uint8_t* color, const uint8_t* pos, const uin
     return cudaGetLastError();
 }
 cudaError_t maxpool2(const ActOut& in, const ActOut& out, int B, int Hin, int Win, int C, cudaStream_t st) {
-    if (in.lo || out.lo || !in.f32 != !out.f32) return cudaErrorInvalidValue;
+    if (in.lo || out.lo || !in.f32 != !out.f32 || in.bf16 != out.bf16) return cudaErrorInvalidValue;
     const size_t opix = static_cast<size_t>(B) * (Hin / 2) * (Win / 2);
     if (in.f32)
         maxpool2_f32_kernel<<<blocks_for(opix * (C / 4), 256), 256, 0, st>>>(in.f32 + in.choff, in.pitch, B, Hin, Win, C,
                                                                              out.f32 + out.choff, out.pitch);
     else
-        maxpool2_kernel<<<blocks_for(opix * (C / 8), 256), 256, 0, st>>>(in.hi + in.choff, in.pitch, B, Hin, Win, C,
-                                                                         out.hi + out.choff, out.pitch);
+        (in.bf16 ? maxpool2_kernel<__nv_bfloat16> : maxpool2_kernel<__half>)<<<blocks_for(opix * (C / 8), 256), 256, 0, st>>>(
+            in.hi + in.choff, in.pitch, B, Hin, Win, C, out.hi + out.choff, out.pitch);
     return cudaGetLastError();
 }
 cudaError_t to_image_space(const float* x, uint8_t* out, size_t n, cudaStream_t st) {

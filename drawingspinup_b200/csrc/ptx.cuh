@@ -2,6 +2,7 @@
 // cp.async, ldmatrix, proxy fences, mbarriers and 1-D bulk copies, and warpgroup MMA (wgmma) with shared-memory operand
 // descriptors or A in registers.
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
 
@@ -118,95 +119,104 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[64 x N] += A[64 x 16] * B[16 x N]; fp16 operands from shared memory (both K-major), fp32 accumulators in registers.
+// D[64 x N] += A[64 x 16] * B[16 x N]; 16-bit operands of type T (__half: .f16, __nv_bfloat16: .bf16) from shared memory
+// (both K-major), fp32 accumulators in registers.
 // Thread t of the warpgroup holds d[i] = D[16 * (t / 32) + (t % 32) / 4 + 8 * ((i >> 1) & 1)][8 * (i >> 2) + 2 * (t % 4) + (i & 1)].
-template <int N>
+// mma_rs: A from registers (RS form), a[0..3] = the warp's 16 x 16 A fragment (rows l/4 and l/4 + 8, as ldsm_x4 returns it).
+template <int N, typename T>
 struct Wgmma;
 
-template <>
-struct Wgmma<32> {
-    __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-            : "l"(a), "l"(b));
-    }
-    // A from registers (RS form): a[0..3] = the warp's 16 x 16 A fragment (rows l/4 and l/4 + 8, as ldsm_x4 returns it)
-    __device__ __forceinline__ static void mma_rs(float* d, const uint32_t* a, uint64_t b) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
-    }
-};
+#define DSU_WGMMA_N32(T, TY) \
+    template <> \
+    struct Wgmma<32, T> { \
+        __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b) { \
+            asm volatile( \
+                "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t" \
+                "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " " \
+                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}" \
+                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+                  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) \
+                : "l"(a), "l"(b)); \
+        } \
+        __device__ __forceinline__ static void mma_rs(float* d, const uint32_t* a, uint64_t b) { \
+            asm volatile( \
+                "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t" \
+                "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " " \
+                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}" \
+                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+                  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) \
+                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b)); \
+        } \
+    };
 
-template <>
-struct Wgmma<64> {
-    __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-            : "l"(a), "l"(b));
-    }
-    // A from registers (RS form): a[0..3] = the warp's 16 x 16 A fragment (rows l/4 and l/4 + 8, as ldsm_x4 returns it)
-    __device__ __forceinline__ static void mma_rs(float* d, const uint32_t* a, uint64_t b) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
-    }
-};
+#define DSU_WGMMA_N64(T, TY) \
+    template <> \
+    struct Wgmma<64, T> { \
+        __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b) { \
+            asm volatile( \
+                "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t" \
+                "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " " \
+                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}" \
+                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+                  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+                  "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+                  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+                : "l"(a), "l"(b)); \
+        } \
+        __device__ __forceinline__ static void mma_rs(float* d, const uint32_t* a, uint64_t b) { \
+            asm volatile( \
+                "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t" \
+                "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " " \
+                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}" \
+                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+                  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+                  "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+                  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b)); \
+        } \
+    };
 
-template <>
-struct Wgmma<128> {
-    __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-            : "l"(a), "l"(b));
-    }
-    // A from registers (RS form): a[0..3] = the warp's 16 x 16 A fragment (rows l/4 and l/4 + 8, as ldsm_x4 returns it)
-    __device__ __forceinline__ static void mma_rs(float* d, const uint32_t* a, uint64_t b) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
-    }
-};
+#define DSU_WGMMA_N128(T, TY) \
+    template <> \
+    struct Wgmma<128, T> { \
+        __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b) { \
+            asm volatile( \
+                "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t" \
+                "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " " \
+                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}" \
+                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+                  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+                  "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+                  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+                  "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+                  "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+                  "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+                  "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+                : "l"(a), "l"(b)); \
+        } \
+        __device__ __forceinline__ static void mma_rs(float* d, const uint32_t* a, uint64_t b) { \
+            asm volatile( \
+                "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t" \
+                "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " " \
+                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}" \
+                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+                  "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+                  "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+                  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+                  "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+                  "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+                  "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+                  "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b)); \
+        } \
+    };
+
+#define DSU_WGMMA(T, TY) DSU_WGMMA_N32(T, TY) DSU_WGMMA_N64(T, TY) DSU_WGMMA_N128(T, TY)
+DSU_WGMMA(__half, "f16")
+DSU_WGMMA(__nv_bfloat16, "bf16")
+#undef DSU_WGMMA
+#undef DSU_WGMMA_N32
+#undef DSU_WGMMA_N64
+#undef DSU_WGMMA_N128
 
 }  // namespace dsu
