@@ -17,10 +17,13 @@ KIND_GENERATORJ = 2
 PREC_FP16 = 0
 PREC_FP16X3 = 1
 PREC_BF16 = 2
+PREC_BF16X3 = 3
 NORM_NONE, NORM_BATCH, NORM_INSTANCE = 0, 1, 2
 E_NOTIMPL = -4
 
 PRECISIONS = {"fp16": PREC_FP16, "fp16x3": PREC_FP16X3, "bf16": PREC_BF16}
+# every precision mode the engine accepts, by name: PRECISIONS and split bf16 (hi + lo bf16 operands, 3 MMA passes)
+MODES = {**PRECISIONS, "bf16x3": PREC_BF16X3}
 
 
 class DsuConfig(C.Structure):

@@ -1,9 +1,10 @@
 // Activation storage: how a value that crosses a kernel boundary sits in HBM (NHWC, DESIGN section 3), and the device
-// helpers that convert and store it.  A buffer holds one of four forms, chosen per handle by engine.cu act_out:
+// helpers that convert and store it.  A buffer holds one of five forms, chosen per handle by engine.cu act_out:
 //   * fp16, one plane (fp16 mode);
 //   * bf16, one plane (bf16 mode): the same 2-byte elements, pitch and padding as the fp16 plane;
 //   * fp16 hi = fp16(v) and lo = fp16(v - hi), two planes (split-fp16 stage 2);
-//   * fp32 (split-fp16 stage 1: the RIC producers blend in fp32 and split after the blend).
+//   * bf16 hi = bf16(v) and lo = bf16(v - hi), two planes (split-bf16 stage 2), laid out like the split-fp16 planes;
+//   * fp32 (stage 1 of both split modes: the RIC producers blend in fp32 and split after the blend).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -15,7 +16,7 @@
 namespace dsu {
 
 // Where a kernel stores channel c of pixel p: element p * pitch + choff + c of `f32` when it is non-null, else of `hi`
-// (and of `lo` when non-null).  All null: no store.  `bf16`: the `hi` plane holds bf16 bits (never with a lo plane).
+// (and of `lo` when non-null).  All null: no store.  `bf16`: the `hi` (and `lo`) plane holds bf16 bits, not fp16.
 struct ActOut {
     __half* hi;
     __half* lo;
@@ -50,16 +51,18 @@ template <typename T>
 __device__ __forceinline__ uint4 pack8(const float* f) {
     return make_uint4(pack_h2<T>(f[0], f[1]), pack_h2<T>(f[2], f[3]), pack_h2<T>(f[4], f[5]), pack_h2<T>(f[6], f[7]));
 }
-// 2 fp32 -> packed fp16 hi and residual lo = fp16(v - hi)
+// 2 fp32 -> packed T hi and residual lo = T(v - hi), T = __half (split fp16) or __nv_bfloat16 (split bf16)
+template <typename T>
 __device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-    hi = pack_h2<__half>(a, b);
-    const float2 r = unpack_h2<__half>(hi);
-    lo = pack_h2<__half>(a - r.x, b - r.y);
+    hi = pack_h2<T>(a, b);
+    const float2 r = unpack_h2<T>(hi);
+    lo = pack_h2<T>(a - r.x, b - r.y);
 }
-// 8 fp32 -> packed fp16 hi and residual lo, two channels at a time
+// 8 fp32 -> packed T hi and residual lo, two channels at a time
+template <typename T>
 __device__ __forceinline__ void split8(const float* f, uint4& hi, uint4& lo) {
-    split2(f[0], f[1], hi.x, lo.x); split2(f[2], f[3], hi.y, lo.y);
-    split2(f[4], f[5], hi.z, lo.z); split2(f[6], f[7], hi.w, lo.w);
+    split2<T>(f[0], f[1], hi.x, lo.x); split2<T>(f[2], f[3], hi.y, lo.y);
+    split2<T>(f[4], f[5], hi.z, lo.z); split2<T>(f[6], f[7], hi.w, lo.w);
 }
 
 // exact fp32 -> uint8 of custom_transforms.py:7-8: ((clip(x,-1,1)+1)/2*255) truncated, fp32 ops in order
@@ -86,8 +89,13 @@ __device__ __forceinline__ void store_act(const ActOut& o, size_t pix, int c, co
     } else if (o.hi) {
         if (kLo && o.lo) {
             uint4 h[N / 8], l[N / 8];
+            if (o.bf16) {
 #pragma unroll
-            for (int q = 0; q < N / 8; ++q) split8(f + 8 * q, h[q], l[q]);
+                for (int q = 0; q < N / 8; ++q) split8<__nv_bfloat16>(f + 8 * q, h[q], l[q]);
+            } else {
+#pragma unroll
+                for (int q = 0; q < N / 8; ++q) split8<__half>(f + 8 * q, h[q], l[q]);
+            }
 #pragma unroll
             for (int q = 0; q < N / 8; ++q) { reinterpret_cast<uint4*>(o.hi + i)[q] = h[q]; reinterpret_cast<uint4*>(o.lo + i)[q] = l[q]; }
         } else if (o.bf16) {

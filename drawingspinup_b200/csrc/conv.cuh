@@ -19,7 +19,7 @@ constexpr int kStages = 4;      // A + B ring depth; chunk q + 2 is loaded while
 constexpr int kMaxSeg = 6;      // concat segments (second half = lo planes in exact mode)
 constexpr int kChannelAlign = 32;   // stored activation widths are multiples of this (the epilogue's 32-column batches)
 // widest output-channel piece of one launch (the widest Cout launch_mode instantiates in that precision; fp16 and bf16
-// share the single-pass value)
+// share the single-pass value, split fp16 and split bf16 the split one)
 constexpr int kMaxPiece(bool exact) { return exact ? 128 : 256; }
 
 // Which mainloop and A producer a convolution launch runs.  This is the one statement of the rule (engine.cu compile_layer
@@ -31,7 +31,7 @@ constexpr int kMaxPiece(bool exact) { return exact ? 128 : 256; }
 // The run-time alternatives use the same chunks and weight packing as the plan-time mode.
 //
 // Output-channel pieces.  Every activation is stored with its width rounded up to a multiple of 32 (kChannelAlign; the
-// padding channels hold exact zeros).  A layer whose padded width exceeds kMaxPiece (128 in split fp16, 256 in fp16 / bf16) runs as
+// padding channels hold exact zeros).  A layer whose padded width exceeds kMaxPiece (128 in split fp16 / bf16, 256 in fp16 / bf16) runs as
 // several launches over contiguous channel ranges, widest first (split-fp16 160 -> 128 + 32, fp16 384 -> 256 + 128), each
 // with its own weight tiles, affine and output channel offset; the residual stream and the instance-norm scratch keep the
 // layer's full pitch (EpiParams::resid_pitch).  The mode above is decided once per layer on its padded width, so every piece
@@ -95,7 +95,7 @@ struct ConvParams {
     int Hv, Wv;             // virtual conv-input geometry = (Hin << up, Win << up)
     ConvMode mode;
     int stride, up, exact;
-    int bf16;               // single-pass bf16 operands (exact = 0): the kernels' element type is __nv_bfloat16, not __half
+    int bf16;               // bf16 operands, single pass or split (exact): the kernels' element type is __nv_bfloat16, not __half
     int nchunks, nblocks, Cout;
     int b_bytes;            // bytes per B stage = Cout x 128 (one chunk's weight tile in wpack)
     // K-step masks as launch constants so the issuing warpgroups stay uniform (kmask: which of the 4 K=16 steps are
@@ -110,7 +110,7 @@ struct ConvParams {
     const float2* ric_lyx;  // [Hout*Wout][8]
     const uint8_t* ric_oct; // [Hout*Wout]
     const uint2* ric_wh;    // [Hout*Wout][8] the 4 bilinear weights of each rotated tap as fp16 {w00,w01 | w10,w11} (packed-half2 blend,
-                            // fp16 mode; split fp16 and bf16 blend in fp32 from ric_lyx)
+                            // fp16 mode; split fp16, bf16 and split bf16 blend in fp32 from ric_lyx)
     EpiParams epi;
     // sub-pixel class of a fused nearest-x2 + 3x3 convolution: the launch is a 2x2 convolution over the LOW-resolution
     // source whose output pixel (oy, ox) of the Hout x Wout grid lands at (2*oy + sub_py, 2*ox + sub_px) of the

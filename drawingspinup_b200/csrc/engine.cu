@@ -1,9 +1,9 @@
 // Network planner + C ABI (include/dsu_b200.h) of the stylization engine.
 //
 // Turns the constructor arguments of GeneratorJ / GeneratorJ_RIC (training/models.py:24-111,
-// 200-291) and a loaded state dict into a list of fused convolution launches (conv_wgmma.cu):
+// 200-291) and a loaded state dict into a list of fused convolution launches (conv_wgmma.cuh):
 // BatchNorm (eval) is folded into per-channel scale/shift, conv weights are rounded to fp16
-// (hi [+lo]) or bf16 and pre-swizzled into tensor-core tiles, skip connections / nearest-x2 upsampling /
+// (hi [+lo]) or bf16 (hi [+lo]) and pre-swizzled into tensor-core tiles, skip connections / nearest-x2 upsampling /
 // stride / concat become slot tables, and the dead stage-1 smoother conv (models.py:348-350) is
 // dropped.  Activations live in NHWC workspace buffers owned by the handle, in one of the forms of act.cuh.
 #include <cuda_bf16.h>
@@ -143,14 +143,14 @@ struct dsu_engine {
     Knobs knobs;
     int cin_pad = 8;
     bool exact = false, finalized = false;
-    bool bf16 = false;        // DSU_PREC_BF16: bf16 weights and activation planes (single pass, the fp16 plan)
+    bool bf16 = false;        // DSU_PREC_BF16 / BF16X3: bf16 weights and activation planes (the fp16 / split-fp16 plan)
     std::map<std::string, std::vector<int64_t>> expected;
     std::vector<std::string> expected_order;
     std::map<std::string, std::vector<float>> w;
     std::set<std::string> loaded;
     std::vector<LayerDef> layers;
     std::vector<Step> steps;
-    bool f32_acts = false;    // stage 1 in split-fp16 mode: activation buffers hold fp32 instead of fp16 hi + lo planes
+    bool f32_acts = false;    // stage 1 in a split mode: activation buffers hold fp32 instead of hi + lo planes
     int buf_level[NBUF]{}, buf_C[NBUF]{};
     bool buf_used[NBUF]{};
     float* d_b12 = nullptr;
@@ -495,7 +495,9 @@ int compile_layer(dsu_engine* E, LayerDef& L) {
                 for (int ci = 0; ci < h.nvalid; ++ci) {
                     const float wv = Wt[((static_cast<size_t>(L.n0 + o) * cin_total + h.wch + ci) * k + h.kh) * k + h.kw];
                     if (E->bf16) {
-                        put(off, o, d, ci, __float2bfloat16_rn(wv));
+                        const __nv_bfloat16 wb = __float2bfloat16_rn(wv);
+                        put(off, o, d, ci, wb);
+                        if (exact) put(off, o, d + 4, ci, __float2bfloat16_rn(wv - __bfloat162float(wb)));
                         continue;
                     }
                     const __half wh = __float2half_rn(wv);
@@ -874,7 +876,8 @@ int dsu_create(const dsu_config* cfg, dsu_handle* out) {
     if (cfg->kind != DSU_KIND_GENERATORJ_RIC && cfg->kind != DSU_KIND_GENERATORJ)
         return fail(DSU_E_INVALID, "kind must be DSU_KIND_GENERATORJ_RIC or DSU_KIND_GENERATORJ");
     if (cfg->norm != DSU_NORM_BATCH && cfg->norm != DSU_NORM_NONE && cfg->norm != DSU_NORM_INSTANCE) return fail(DSU_E_INVALID, "bad norm");
-    if (cfg->precision != DSU_PREC_FP16 && cfg->precision != DSU_PREC_FP16X3 && cfg->precision != DSU_PREC_BF16)
+    if (cfg->precision != DSU_PREC_FP16 && cfg->precision != DSU_PREC_FP16X3 && cfg->precision != DSU_PREC_BF16 &&
+        cfg->precision != DSU_PREC_BF16X3)
         return fail(DSU_E_INVALID, "bad precision");
     if (cfg->input_channels < 1 || cfg->input_channels > 16) return fail(DSU_E_INVALID, "input_channels must be in [1,16]");
     if (cfg->resnet_blocks < 0 || cfg->resnet_blocks > 64) return fail(DSU_E_INVALID, "resnet_blocks out of range");
@@ -895,8 +898,8 @@ int dsu_create(const dsu_config* cfg, dsu_handle* out) {
     E->cfg = *cfg;
     E->knobs = knobs_from_env();
     E->cin_pad = (cfg->input_channels + 7) / 8 * 8;
-    E->exact = cfg->precision == DSU_PREC_FP16X3;
-    E->bf16 = cfg->precision == DSU_PREC_BF16;
+    E->exact = cfg->precision == DSU_PREC_FP16X3 || cfg->precision == DSU_PREC_BF16X3;
+    E->bf16 = cfg->precision == DSU_PREC_BF16 || cfg->precision == DSU_PREC_BF16X3;
     E->f32_acts = cfg->kind == DSU_KIND_GENERATORJ_RIC && E->exact;
     int rc = build_plan(E);
     if (rc) { delete E; return rc; }

@@ -15,7 +15,7 @@ cudaError_t ingest_f32(const float* x, int B, int cin, int cpad, int H, int W, c
 cudaError_t ingest_u8(const uint8_t* color, const uint8_t* pos, const uint8_t* edge, int derive_edge, bool has_mask, bool has_pos,
                       int B, int H, int W, const ActOut& out, cudaStream_t st);
 // 2x2 / stride 2 max-pool of C channels from `in` to `out`, both fp16, both bf16 or both fp32; a lo plane is an error (the
-// split-fp16 mode pools only in stage 1, whose activations are fp32)
+// split modes pool only in stage 1, whose activations are fp32)
 cudaError_t maxpool2(const ActOut& in, const ActOut& out, int B, int Hin, int Win, int C, cudaStream_t st);
 cudaError_t frames_to_tensor(const uint8_t* color, const uint8_t* pos, const uint8_t* edge, int B, int H, int W,
                              float* pre, float* mask, cudaStream_t st);

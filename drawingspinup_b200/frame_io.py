@@ -42,7 +42,7 @@ import numpy as np
 import torch
 from PIL import Image
 
-from . import layout
+from . import capi, layout
 
 # result folders of the default flags (no --no_* flag); every other name comes from layout.log_name / result_name
 STAGE1_RES, STAGE2_RES = layout.result_name(1), layout.result_name(2)
@@ -294,7 +294,7 @@ def main(argv=None) -> int:
     ap.add_argument("--root", default="../dataset/AnimatedDrawings/preprocessed", help="root_dir of the reference configs")
     ap.add_argument("--uid", required=True)
     ap.add_argument("--checkpoint_id", type=int, default=99999)
-    ap.add_argument("--precision", default="fp16x3", choices=["fp16", "fp16x3", "bf16"])
+    ap.add_argument("--precision", default="fp16x3", choices=sorted(capi.MODES))
     ap.add_argument("--stage", type=int, choices=[1, 2], default=None,
                     help="run test_stage1.py (1) or test_stage2.py (2) alone (default: both, chained)")
     ap.add_argument("--no_mask", action="store_true", help="checkpoints trained without the mask channel")

@@ -109,8 +109,8 @@ class _Generator(nn.Module):
         # flag is kept for callers that request it explicitly.
         self.deterministic = bool(int(os.environ.get("DSU_DETERMINISTIC", "0"))) if deterministic is None else bool(deterministic)
         self.precision = precision or os.environ.get("DSU_PRECISION", "fp16x3")
-        if self.precision not in capi.PRECISIONS:
-            raise ValueError("precision must be one of %s" % sorted(capi.PRECISIONS))
+        if self.precision not in capi.MODES:
+            raise ValueError("precision must be one of %s" % sorted(capi.MODES))
         f, k0, bn = self.filters, self._FIRST_K, norm_layer == 'batch_norm'
 
         def relu_layer(cin, cout, k):
@@ -195,7 +195,7 @@ class _Generator(nn.Module):
             cfg.tanh = int(self.tanh)
             cfg.append_smoothers = int(self.append_smoothers)
             cfg.norm = {'batch_norm': capi.NORM_BATCH, 'instance_norm': capi.NORM_INSTANCE}.get(self.norm_layer, capi.NORM_NONE)
-            cfg.precision = capi.PRECISIONS[self.precision]
+            cfg.precision = capi.MODES[self.precision]
             cfg.device = idx
             h = C.c_void_p()
             capi.check(lib.dsu_create(C.byref(cfg), C.byref(h)), "dsu_create")

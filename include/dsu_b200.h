@@ -39,6 +39,9 @@ extern "C" {
 #define DSU_PREC_FP16 0     /* fp16 operands, fp32 accumulate (1 MMA pass) */
 #define DSU_PREC_FP16X3 1   /* split fp16 hi+lo operands, 3 MMA passes: fp32-grade, meets 1e-3 parity */
 #define DSU_PREC_BF16 2     /* bf16 operands, fp32 accumulate (1 MMA pass): fp32's exponent range at fp16's width and rate */
+/* split bf16 hi+lo operands, 3 MMA passes: a 16-bit significand with fp32's exponent range (value 3: the split of
+ * DSU_PREC_FP16X3 combined with the element type of DSU_PREC_BF16) */
+#define DSU_PREC_BF16X3 (DSU_PREC_BF16 | DSU_PREC_FP16X3)
 
 #define DSU_NORM_NONE 0
 #define DSU_NORM_BATCH 1
@@ -128,8 +131,8 @@ double dsu_forward_flops(dsu_handle h, int32_t B, int32_t H, int32_t W);
 int dsu_profile_forward(dsu_handle h, int32_t B, int32_t H, int32_t W, int32_t reps, void* stream,
                         double* ms_out, double* flops_out, int32_t capacity);
 /* Name of launch i of a forward ("ingest", "conv0", "maxpool", "resnets.3.conv_1", ...).  A layer wider than one launch
- * computes (128 channels in DSU_PREC_FP16X3, 256 in DSU_PREC_FP16 and DSU_PREC_BF16) runs as output-channel pieces "<layer>.n0", "<layer>.n1",
- * ...; a final layer in pieces is followed by "conv_12", which sums their conv_12 partial dot products. */
+ * computes (128 channels in DSU_PREC_FP16X3 and DSU_PREC_BF16X3, 256 in DSU_PREC_FP16 and DSU_PREC_BF16) runs as
+ * output-channel pieces "<layer>.n0", "<layer>.n1", ...; a final layer in pieces is followed by "conv_12", which sums their conv_12 partial dot products. */
 const char* dsu_step_name(dsu_handle h, int32_t index);
 /* Mainloop launch i runs with the handle's current plan and knobs: "halo" (A fragments from a shared-memory input halo),
  * "tap" (A tiles gathered per tap), "ric_halo" (stage-1 deformable, stencil and corners from shared memory), "ric" (stage-1
@@ -153,9 +156,9 @@ int dsu_compose_rgba(const float* y_dev, const float* mask_dev, int32_t B, int32
 int dsu_pos2edge(const uint8_t* pos_dev, int32_t B, int32_t H, int32_t W, uint8_t* edge_dev, void* stream);
 
 /* Test hook: copy an internal activation buffer of the last forward to the host (synchronous).
- * buffer: 0 SK0(o0|x) 1 P0 2 O1 3 P1 4 O2 5 T 6 U 7 V2 8 V1 9 C11 10 S0 (fp16 NHWC; bf16 bits in plane 0 for a
- * DSU_PREC_BF16 handle; fp32 in stage 1 of DSU_PREC_FP16X3), 100 = fp32 residual stream; plane 0 = hi, 1 = lo
- * (DSU_PREC_FP16X3 stage 2 only).  Copies min(bytes, buffer size). */
+ * buffer: 0 SK0(o0|x) 1 P0 2 O1 3 P1 4 O2 5 T 6 U 7 V2 8 V1 9 C11 10 S0 (fp16 NHWC; bf16 bits for a DSU_PREC_BF16 or
+ * DSU_PREC_BF16X3 handle; fp32 in stage 1 of DSU_PREC_FP16X3 and DSU_PREC_BF16X3), 100 = fp32 residual stream;
+ * plane 0 = hi, 1 = lo (stage 2 of DSU_PREC_FP16X3 and DSU_PREC_BF16X3 only).  Copies min(bytes, buffer size). */
 int dsu_debug_read(dsu_handle h, int32_t buffer, int32_t plane, void* dst_host, size_t bytes);
 
 #ifdef __cplusplus

@@ -1,9 +1,9 @@
-"""The three precision modes side by side on bench.py's c2 workload: 64 synthetic frames of 512 x 512 through stage 1 and
+"""The four precision modes side by side on bench.py's c2 workload: 64 synthetic frames of 512 x 512 through stage 1 and
 stage 2, batch 16, the seeded weights and frames bench.py builds.
 
     python tools/precision_modes.py [--rounds 2] [--steps 3] [--warmup 2]
 
-Per mode (fp16x3, fp16, bf16), alternated in one process for ``--rounds`` rounds: frames/s of the whole 64-frame step
+Per mode (fp16x3, fp16, bf16, bf16x3), alternated in one process for ``--rounds`` rounds: frames/s of the whole 64-frame step
 (device-resident stacks, CUDA events), stage-1 and stage-2 milliseconds per 16-frame batch (each stage timed alone), and
 the max-abs error of each stage against the fp32 reference forward on the GPU (oracle port, TF32 off) on bench.py's
 parity-gate frame.  Prints one JSON line with the GPU's name and power limit read in the same run; the per-round numbers
@@ -23,7 +23,7 @@ import bench  # noqa: E402
 from drawingspinup_b200 import synth  # noqa: E402
 from drawingspinup_b200.pipeline import StylizationPipeline  # noqa: E402
 
-MODES = ("fp16x3", "fp16", "bf16")
+MODES = ("fp16x3", "fp16", "bf16", "bf16x3")
 SIZE, FRAMES, BATCH, SEED = 512, 64, 16, 1234
 
 
@@ -84,6 +84,7 @@ def main():
                            "stage2_ms_per_batch": min(r["stage2_ms_per_batch"] for r in rounds[m]),
                            "max_abs_err": errs[m], "rounds": rounds[m]}
     out["bf16_vs_fp16_frames_per_s"] = out["modes"]["bf16"]["frames_per_s"] / out["modes"]["fp16"]["frames_per_s"]
+    out["bf16x3_vs_fp16x3_frames_per_s"] = out["modes"]["bf16x3"]["frames_per_s"] / out["modes"]["fp16x3"]["frames_per_s"]
     print(json.dumps(out), flush=True)
 
 
